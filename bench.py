@@ -152,21 +152,18 @@ class ClockSampler:
                 "samples": len(sm), "reasons": sorted(reasons)}
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu --set full captures (profiles/)
-TRAFFIC_NCU = {"dlinear_chain": 398770688}  # profiles/r1_ncu_summary.md (r1b_dlinear_chain_full.ncu-rep, mean of 2 launches)
-
-
 def measured_peaks():
+    # fallback: NVIDIA's H100 SXM data sheet (3.35 TB/s HBM3, 989 dense BF16 TFLOP/s at up to 700 W), never reached
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1590.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, "data sheet"
 
 
 # ------------------------------------------------------------------------------------------------
 # roofline probe: the dominant kernel timed live (CUDA events, kernel launched alone in a loop over
-# all decoder layers' weights so the working set (>= 4 GB) is far larger than the 126 MB L2)
+# all decoder layers' weights so the working set (>= 4 GB) is far larger than the 50 MB L2)
 # ------------------------------------------------------------------------------------------------
 def roofline_probe(model, spec, geom):
     from u2tokenizer_b200 import ops
@@ -174,7 +171,7 @@ def roofline_probe(model, spec, geom):
     hbm, tf, src = measured_peaks()
     if spec["mode"] == "generate":
         # dominant kernel of the generate workload: the decode-step linear chain launch
-        # (dlinear_tcgen05_kernel: o_proj -> gate|up -> down -> next qkv in ONE launch, 386 MB of weights for 8B)
+        # (dlinear_wgmma_kernel: o_proj -> gate|up -> down -> next qkv in ONE launch, 386 MB of weights for 8B)
         B = spec["batch"]
         hq, hkv, dh, I, E = (geom.num_attention_heads, geom.num_key_value_heads, geom.head_dim, geom.intermediate_size,
                              geom.hidden_size)
@@ -217,11 +214,11 @@ def roofline_probe(model, spec, geom):
         act_bytes = 2 * B * (hq * dh + 3 * E + 2 * E + 2 * I + 2 * E + nq)  # activations in/out of the four linears
         alg_bytes = w_bytes + act_bytes
         ach = alg_bytes / sec / 1e9
-        return {"bound": "hbm", "kernel": "dlinear_tcgen05_kernel<128> (decode chain: o_proj+gate|up+down+qkv in one launch)",
+        return {"bound": "hbm", "kernel": "dlinear_wgmma_kernel<128> (decode chain: o_proj+gate|up+down+qkv in one launch)",
                 "achieved": round(ach, 1), "peak": hbm, "unit": "GB/s", "frac": round(ach / hbm, 4),
-                "traffic": TRAFFIC_NCU.get("dlinear_chain"), "peak_source": src, "bytes_per_launch": alg_bytes,
+                "peak_source": src, "bytes_per_launch": alg_bytes,
                 "us_per_launch": round(sec * 1e6, 2),
-                "note": "timed live with CUDA events over all layers' weights (13.9 GB working set >> 126 MB L2)"}
+                "note": "timed live with CUDA events over all layers' weights (13.9 GB working set >> 50 MB L2)"}
     # forward workloads: the ViT MLP GEMM (largest share of tensor work)
     Fr = spec["batch"] * spec["frames"]
     M = Fr * 2056
@@ -248,7 +245,7 @@ def roofline_probe(model, spec, geom):
     sec = e0.elapsed_time(e1) / 1e3 / 30
     fl = 2.0 * M * geom.vit_mlp * geom.vit_hidden
     ach = fl / sec / 1e12
-    return {"bound": "tensor", "kernel": "gemm_bf16_tcgen05_kernel (ViT MLP fc1 + GELU)", "achieved": round(ach, 1), "peak": tf,
+    return {"bound": "tensor", "kernel": "gemm_bf16_wgmma_kernel (ViT MLP fc1 + GELU)", "achieved": round(ach, 1), "peak": tf,
             "unit": "TFLOP/s", "frac": round(ach / tf, 4), "traffic": None, "peak_source": src,
             "flops_per_launch": fl, "us_per_launch": round(sec * 1e6, 2)}
 
@@ -263,7 +260,7 @@ def extra_rooflines(model, spec, geom):
     ev = lambda: torch.cuda.Event(enable_timing=True)
     # --- the WHOLE 3-D patch-embedding op (SURVEY.md section 8d: 97.0 MB of algorithmic traffic per 256^3 volume = fp32 volume in,
     # bf16 tokens out, weights once; 25.8 GFLOP): brick gather + GEMM (+bias +position table, rows placed behind the cls
-    # row) + cls / padding rows, 32 frames = 4 volumes per pass, two buffer sets alternated (537 MB >> 126 MB L2)
+    # row) + cls / padding rows, 32 frames = 4 volumes per pass, two buffer sets alternated (537 MB >> 50 MB L2)
     Fr = 32
     D0, D1, D2 = geom.image_size
     P, Hd, pd = geom.n_patches, geom.vit_hidden, geom.patch_dim
@@ -304,9 +301,9 @@ def extra_rooflines(model, spec, geom):
     us_unfused = timed_us(embed_unfused) if fused else us_op
     by_op = Fr * (D0 * D1 * D2 * 4 + P * Hd * 2) + (pd * Hd + P * Hd + Hd) * 2
     fl_op = 2.0 * Fr * P * pd * Hd
-    out.append({"kernel": ("3-D patch embedding, whole op (patch_embed_tcgen05_kernel: 5-D TMA slabs -> in-smem fp32->bf16 A operand -> "
-                           "tcgen05, bias + position epilogue; + vit_frame_rows_kernel)") if fused else
-                          "3-D patch embedding, whole op (patchify_tma_kernel + gemm_bf16_tcgen05_kernel<256> + vit_frame_rows_kernel)",
+    out.append({"kernel": ("3-D patch embedding, whole op (patch_embed_wgmma_kernel: 5-D TMA slabs -> in-smem fp32->bf16 A operand -> "
+                           "wgmma, bias + position epilogue; + vit_frame_rows_kernel)") if fused else
+                          "3-D patch embedding, whole op (patchify_tma_kernel + gemm_bf16_wgmma_kernel<128> + vit_frame_rows_kernel)",
                 "bound": "hbm / tensor (arithmetic intensity 266 FLOP/B vs ridge 218)", "achieved": round(by_op / us_op / 1e3, 1),
                 "peak": hbm, "unit": "GB/s", "frac": round(by_op / us_op / 1e3 / hbm, 4), "bytes_per_launch": by_op,
                 "us_per_launch": round(us_op, 2), "tensor_achieved_tflops": round(fl_op / us_op / 1e6, 1),
@@ -334,7 +331,7 @@ def extra_rooflines(model, spec, geom):
     torch.cuda.synchronize()
     sec = e0.elapsed_time(e1) / 1e3 / nl
     fl = 2.0 * M * 2 * I * E
-    out.append({"kernel": f"gemm_bf16_tcgen05_kernel<256> (decoder prefill gate|up, M={M} N={2 * I} K={E})", "bound": "tensor",
+    out.append({"kernel": f"gemm_bf16_wgmma_kernel<128> (decoder prefill gate|up, M={M} N={2 * I} K={E})", "bound": "tensor",
                 "achieved": round(fl / sec / 1e12, 1), "peak": tf, "unit": "TFLOP/s", "frac": round(fl / sec / 1e12 / tf, 4),
                 "flops_per_launch": fl, "us_per_launch": round(sec * 1e6, 2), "peak_source": src})
     return out
@@ -635,6 +632,8 @@ def train_main(args, cfg, geom, spec, base, rank, local_rank, world, dist):
     clocks = sampler.stop() if rank == 0 else None
     if rank != 0:
         return
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"loss": out})
     B = spec["batch"] if spec["mode"] != "dpo" else 1   # DPO: one study per pair
     n_tok = batch[1].shape[0] * batch[1].shape[1]
     fwd_fl, step_fl = train_flops(geom, batch[1].shape[0], spec["frames"], spec["seq"], spec["lt"])
@@ -649,7 +648,7 @@ def train_main(args, cfg, geom, spec, base, rank, local_rank, world, dist):
                   "phases_ms": phases, "loss": [float(x) for x in out.flatten()[:3]] if out.numel() > 1 else float(out),
                   "optimizer": f"AdamW, ZeRO-1 over {world} rank(s): fp32 master, {str(mom).split('.')[-1]} moments, "
                                f"{te.lay.n_buckets} gradient buckets of {te.lay.bucket} bf16 elements, max_grad_norm 1.0",
-                  "roofline": {"bound": "tensor", "kernel": "training step (all tcgen05 GEMMs: forward, dgrad, wgrad, attention)",
+                  "roofline": {"bound": "tensor", "kernel": "training step (all wgmma GEMMs: forward, dgrad, wgrad, attention)",
                                "achieved": round(step_fl / (compute_ms / 1e3) / 1e12, 1), "peak": tf, "unit": "TFLOP/s",
                                "frac": round(step_fl / (compute_ms / 1e3) / 1e12 / tf, 4), "traffic": None, "peak_source": src,
                                "flops_per_step": step_fl, "note": "algorithmic FLOPs of forward + backward per rank / (forward + backward ms)"},
@@ -664,10 +663,20 @@ def train_main(args, cfg, geom, spec, base, rank, local_rank, world, dist):
 
 def train_substep(model, rank, local_rank, world, dist, steps=3, warmup=3):
     """cfg 4 training step (2 volumes / GPU, 512-token sequences) on the model the generate benchmark just used: its
-    parameters move into the training engine's flat buffer (no second copy), every rank joins the ZeRO-1 exchange."""
+    parameters move into the training engine's flat buffer (no second copy), every rank joins the ZeRO-1 exchange.
+    The training state costs 4 bytes per parameter on every rank (bf16 weights and gradients) plus 8 / world (fp32
+    master and bf16 moments, sharded): for the 8B model on fewer ranks than that needs (one 80 GB H100 holds 4 + 8
+    bytes x 8.2e9 = 98 GB only with offloading) the step trains mu2-Qwen3-1.7B at the same batch geometry instead."""
     import gc
     from u2tokenizer_b200 import parallel
     cfg4, geom4, spec4 = make_geometry("cfg4")
+    n_par = sum(p.numel() for p in model.parameters())
+    own = n_par * (4 + 8 / world) > 0.6 * torch.cuda.mem_get_info()[1]
+    if own:
+        model.invalidate_engine()
+        cfg_s, geom4, _ = make_geometry("cfg2")
+        spec4 = dict(spec4, model="mu2-Qwen3-1.7B")
+        model = build_model(cfg_s, geom4)
     model.invalidate_engine()
     gc.collect()
     torch.cuda.empty_cache()
@@ -686,7 +695,7 @@ def train_substep(model, rank, local_rank, world, dist, steps=3, warmup=3):
         hbm, tf, src = measured_peaks()
         per = ms / steps
         comp = per - phases["exposed_reduce_scatter"] - phases["clip_adamw"]
-        return {"workload": "cfg4: mu2-Qwen3-8B training step, 2 volumes / GPU (raw depth 64 / 128 / 256 zero-padded to 8 frames), "
+        return {"workload": f"cfg4: {spec4['model']} training step, 2 volumes / GPU (raw depth 64 / 128 / 256 zero-padded to 8 frames), "
                             "512-token sequences, forward + backward + ZeRO-1 (bucketed NCCL reduce-scatter overlapped with the "
                             "backward, sharded fused AdamW, all-gather overlapped with the next forward)",
                 "value": round(world * spec4["batch"] * steps / (ms / 1e3), 4), "unit": "volumes/s", "ms_per_step": round(per, 3),
@@ -705,6 +714,8 @@ def train_substep(model, rank, local_rank, world, dist, steps=3, warmup=3):
         te.tape = []
         del te
         model.eval()
+        if own:
+            del model
         gc.collect()
         torch.cuda.empty_cache()
 
@@ -754,6 +765,15 @@ def cfg2_forward_substep(steps=10, warmup=3):
         torch.cuda.empty_cache()
 
 
+def dump_outputs(d, arrays):
+    """Outputs of the timed path as float64 .npy files, so that two builds can be compared output for output (the inputs
+    and weights are generated from fixed seeds). Token ids are exact in float64."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(d, f"{name}.npy"), t.detach().double().cpu().numpy())
+
+
 # ------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -763,6 +783,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default=os.environ.get("U2_BENCH_WORKLOAD", "cfg3"))
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path returned in its last timed step as DIR/<name>.npy (float64)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -777,7 +799,7 @@ def main():
                                    f"tokens, question pad {spec['lt']}",
                        "batch_per_gpu": spec["batch"], "frames": spec["frames"], "new_tokens": spec["new_tokens"],
                        "parallelism": f"dp{args.gpus} (independent replicas, no data-path collective)",
-                       "l2": "weights (>= 3.4 GB) and volumes (67 MB each) exceed the 126 MB L2; no explicit flush"}}
+                       "l2": "weights (>= 3.4 GB) and volumes (67 MB each) exceed the 50 MB L2; no explicit flush"}}
 
     if args.impl == "reference":
         if rank != 0:
@@ -799,7 +821,7 @@ def main():
         return
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device (B200); there is no CPU path for the product")
+        raise SystemExit("bench.py needs a CUDA device (H100); there is no CPU path for the product")
     torch.cuda.set_device(local_rank)
     dist = None
     if world > 1:
@@ -848,12 +870,14 @@ def main():
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    prof = os.environ.get("U2_PROFILE_TIMED", "0") != "0"  # ncu --profile-from-start off: capture only the timed region
+    prof = os.environ.get("U2_PROFILE_TIMED", "0") != "0"  # cudaProfilerStart/Stop around the timed region only
     if prof:
         torch.cuda.profiler.start()
     ms_dev, launches, res = timed(lambda: run(d_images, d_ids, d_q), args.steps)
     if prof:
         torch.cuda.profiler.stop()
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"generated_ids" if spec["mode"] == "generate" else "next_token_ids": res})
 
     def e2e_step():
         out = run(h_images.cuda(non_blocking=True), h_ids.cuda(non_blocking=True), h_q.cuda(non_blocking=True))
@@ -903,7 +927,7 @@ def main():
         wd.daemon = True
         wd.start()
         try:
-            ts = train_substep(model, rank, local_rank, world, dist)
+            ts = train_substep(model, rank, local_rank, world, dist, steps=args.steps, warmup=args.warmup)
         except Exception as e:
             ts = {"error": repr(e)}
         wd.cancel()
@@ -915,7 +939,7 @@ def main():
         return
     if world == 1 and args.workload == "cfg3" and os.environ.get("U2_BENCH_CFG2", "1") != "0":
         try:
-            out["cfg2_forward"] = cfg2_forward_substep()
+            out["cfg2_forward"] = cfg2_forward_substep(steps=args.steps, warmup=args.warmup)
         except Exception as e:
             out["cfg2_forward"] = {"error": repr(e)}
     if world == 1 and not args.no_cpu_baseline:

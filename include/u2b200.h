@@ -1,5 +1,5 @@
 /*
- * u2b200.h - C ABI of libu2b200.so: the sm_100a kernels behind the mu2-LLM
+ * u2b200.h - C ABI of libu2b200.so: the sm_90a kernels behind the mu2-LLM
  * "visual-tokenize-then-decode" hot path (CT volume -> 3D patch embed -> ViT3D -> spatial-pooling
  * projector -> mu2-Tokenizer -> splice -> Qwen3/Llama decoder forward / greedy decode).
  *
@@ -49,13 +49,13 @@ extern "C" {
 /* Library / device info ----------------------------------------------------------------------- */
 U2_API int u2_version(void);                 /* ABI version, currently 1 */
 U2_API const char* u2_last_error(void);      /* message of the last failing call on this thread */
-U2_API int u2_device_sm_count(void);         /* SMs of the current device (148 on B200), <0 on error */
+U2_API int u2_device_sm_count(void);         /* SMs of the current device (132 on H100), <0 on error */
 
 /* GEMM --------------------------------------------------------------------------------------------
  * For every batch z = (zo, zi):
  *     C[z] (M x N) = act( alpha * A[z] (M x K) * B[z'] (N x K)^T + bias[n] ) + residual
  * A, B are bf16, K-major (row stride lda/ldb elements, multiples of 8) unless a_mn / b_mn say otherwise;
- * fp32 accumulation in TMEM. residual == C (same ld) accumulates into a bf16 C (gradient accumulation).
+ * fp32 accumulation in registers. residual == C (same ld) accumulates into a bf16 C (gradient accumulation).
  * Batch offsets (elements): A: zi*a_stride_zi + zo*a_stride_zo; B: (zi / b_zi_div)*b_stride_zi +
  * zo*b_stride_zo (b_zi_div > 1 shares one B among consecutive inner batches: GQA);
  * C: zi*c_stride_zi + zo*c_stride_zo.
@@ -80,7 +80,7 @@ typedef struct u2_gemm_desc {
   int64_t ldr;
   int32_t res_row_mod;
   int32_t row_div, row_stride, row_off;
-  int32_t block_n;    /* 0 = auto, else 64/128/256 */
+  int32_t block_n;    /* 0 = auto, else 64/128/256 (256: the widest tile, 128 columns on sm_90) */
   /* transposed operands (training: dgrad = dY * W, wgrad = dY^T * X, P^T dO ...): a_mn != 0 -> A is stored
    * [K][M] (element (m, k) at A[k * lda + m]); b_mn != 0 -> B is stored [K][N]. lda / ldb are then the strides
    * between consecutive contraction indices. No transposed copy is made: the tile is loaded MN-major. */
@@ -177,11 +177,13 @@ U2_API int u2_spp_pool_bf16(const void* x, void* out, int64_t frames, int32_t g0
                             int32_t ps, int32_t E, int64_t in_frame_stride, int64_t in_off, int64_t ldx,
                             int32_t sequence, void* stream);
 /* Multi-scale token pooling, scales (1,2,4) over the token dim of x [B, K, E] -> out [B, K+K/2+K/4, E];
- * dynamic != 0: DynamicMultiScalePooling gate (svr.py:126-151) with gate_w [E] fp32, gate_bias scalar and a
- * [B,3] fp32 workspace; dynamic == 0: the plain concat (svr.py:175-184). */
+ * dynamic != 0: DynamicMultiScalePooling gate (svr.py:126-151) with gate_w [E] fp32, gate_bias scalar and an fp32
+ * workspace of u2_multiscale_pool_ws_elems(B, K) floats whose first B*3 hold the gate logits [B,3] on return (the
+ * rest: per-block partial sums, added in a fixed order); dynamic == 0: the plain concat (svr.py:175-184). */
 U2_API int u2_multiscale_pool_bf16(const void* x, void* out, const float* gate_w, float gate_bias,
                                    float* logits_ws, int32_t B, int32_t K, int32_t E, int32_t dynamic,
                                    void* stream);
+U2_API int64_t u2_multiscale_pool_ws_elems(int32_t B, int32_t K);
 /* out[b][l] = vis[b][l-1] for 1 <= l <= n_vis (when vis != NULL) else table[ids[b][l]]
  * (u2_arch.py:118-121: embed_tokens gather + cat splice). ids int64. */
 U2_API int u2_embed_splice_bf16(const int64_t* ids, const void* table, const void* vis, void* out, int32_t B,
@@ -223,7 +225,7 @@ U2_API int u2_decode_attention_bf16(const void* q, const void* k_cache, const vo
 
 /* Decode-step linear (weight streaming, HBM-bound): y[b, n] = sum_k norm(x)[b, k] * w[n, k] (+ residual).
  * CUDA-core variant of the HF decoder Linears (+ Qwen3RMSNorm, modeling_qwen3.py:50-67) at q_len == 1 inside generate()
- * (src/model/language_model/u2llama.py:123-126) for shapes the tcgen05 path does not take (K % 64 != 0).
+ * (src/model/language_model/u2llama.py:123-126) for shapes the wgmma path does not take (K % 64 != 0).
  * B <= 8. norm_gamma != NULL fuses the input RMSNorm; silu_pair != 0 treats rows (2j, 2j+1) of w as
  * (gate_j, up_j) and writes silu(gate) * up (N/2 outputs). */
 typedef struct u2_gemv_desc {
@@ -249,8 +251,10 @@ U2_API int u2_argmax_f32(const float* logits, int64_t* out, uint64_t* scratch, i
  *   else:      y[b, n] = v + residual[b, n];  optionally xg[b, n] = bf16(y * gamma_next[n]) and
  *              ssq_out[b] += sum_n y^2 (prepares the next fused norm); ssq_zero[0..15] is reset to 0.
  * ws: fp32 partial-sum slots (ws_elems floats; u2_dlinear_ws_elems(N, K) gives the size needed by the stream-K
- * schedule): every 32-bit word must hold 0xffffffff ("empty") on entry and does so again on exit;
- * counters: int32 [ceil(N/64)], zero on entry and on exit.
+ * schedule and the per-tile sums of squares behind the slots): every 32-bit word must hold 0xffffffff ("empty") on
+ * entry and does so again on exit;
+ * counters: int32 [ceil(N/64)] (+1 when ssq_out != NULL: the op's tile ticket), zero on entry and on exit.
+ * ssq_out is added in a fixed order, so repeated launches on the same inputs give identical results.
  * Replaces the HF decoder Linears at q_len == 1 (reference u2llama.py:123-126 -> GenerationMixin._sample). */
 #define U2_DLIN_STREAMK128 0
 #define U2_DLIN_TILES64 1
@@ -339,7 +343,7 @@ U2_API int u2_topk_rows_f32(const float* scores, int64_t* out_idx, int32_t rows,
                             int64_t idx_offset_per_row, void* stream);
 
 /* Fused attention forward, head_dim 64, non-causal (ViT3D): out = softmax(q k^T * scale) v, scores never leave
- * the SM (tcgen05: S and PV partials in TMEM, P through swizzled shared memory).
+ * the SM (wgmma: S, P and the running O stay in registers).
  * q [B, Sq, H, 64], k [B, Sk, H, 64], v [B, Sk, H, 64] as strided views (element strides *_sb batch, *_ss token,
  * *_sh head; d contiguous) - typically the three slices of one fused QKV activation; v is consumed as stored (MN-major
  * B operand of the PV product, no transposed copy); out [B, Sq, H*64] (strides out_sb, out_ss). All strides multiples

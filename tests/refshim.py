@@ -1,8 +1,11 @@
-"""Test-only helper: import the REFERENCE modules from /root/reference (authoring container only).
+"""Test-only helper: import the REFERENCE modules from a checkout of the reference project, where one is mounted at
+REF_ROOT, and otherwise serve their recorded outputs (tests/golden/pins/) so that the pins run everywhere.
 
 MONAI 1.3.0 is neither vendored nor installed, so `monai.networks.blocks.{patchembedding,
 transformerblock}` are provided by a small nn.Module restatement registered in sys.modules; the
 reference's own vit.py / u2_arch.py / u2llama.py then import unchanged. Never used by product code.
+
+Recording (needs the reference tree): U2_RECORD_PINS=1 python -m pytest tests/test_oracle_pin.py tests/test_oracle_grad_pin.py
 """
 import os
 import sys
@@ -11,11 +14,25 @@ import types
 import torch
 import torch.nn as nn
 
-REF_ROOT = "/root/reference"
+REF_ROOT = os.environ.get("U2_REFERENCE_ROOT", "/root/reference")
+PIN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "pins")
 
 
 def have_reference() -> bool:
     return os.path.isdir(os.path.join(REF_ROOT, "src", "model"))
+
+
+def pinned(key, compute, keep=None):
+    """(what the reference computes for `key`, complete?). With the reference tree mounted, `compute()` runs it (and with
+    U2_RECORD_PINS=1 stores the result as golden/pins/<key>.pt, reduced by `keep` where the full output would be large);
+    without it, the stored copy is returned: complete unless `keep` reduced it."""
+    if have_reference():
+        out = compute()
+        if os.environ.get("U2_RECORD_PINS") == "1":
+            os.makedirs(PIN_DIR, exist_ok=True)
+            torch.save(keep(out) if keep else out, os.path.join(PIN_DIR, f"{key}.pt"))
+        return out, True
+    return torch.load(os.path.join(PIN_DIR, f"{key}.pt")), keep is None
 
 
 class _PatchEmbeddingBlock(nn.Module):

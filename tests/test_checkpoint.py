@@ -74,7 +74,7 @@ def test_remote_code_round_trip(family, tmp_path, hf_modules):
 
 def test_reference_config_json_is_understood(tmp_path, hf_modules):
     """A config.json with the reference's own field names (enable_rpe instead of attn_type, extra segmentation fields,
-    base_model_tokenizers/Llama-3.2-1B-Instruct/config.json) resolves to the B200 classes once the shims are written."""
+    base_model_tokenizers/Llama-3.2-1B-Instruct/config.json) resolves to the H100 classes once the shims are written."""
     from transformers import AutoConfig
     ref_like = dict(KW)
     ref_like.pop("attn_type")

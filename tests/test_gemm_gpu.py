@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 GEMM (u2_gemm_bf16) against fp32 torch.matmul on the same bf16 inputs."""
+"""Parity of the wgmma GEMM (u2_gemm_bf16) against fp32 torch.matmul on the same bf16 inputs."""
 import pytest
 import torch
 

@@ -270,13 +270,13 @@ def test_argmax():
 @pytest.mark.parametrize("B", [1, 4, 16])
 @pytest.mark.parametrize("N,K", [(4096, 4096), (1000, 320), (6144, 2048), (24576, 4096), (4096, 12288), (151936, 1024)])
 def test_dlinear(B, N, K, sched):
-    """tcgen05 decode linear (swap-AB + stream-K): plain, fused-norm scale, residual + next-norm prep, silu pair."""
+    """wgmma decode linear (swap-AB + stream-K): plain, fused-norm scale, residual + next-norm prep, silu pair."""
     from u2tokenizer_b200 import ops
     g = gen(B * N + K + 1)
     x = torch.randn(B, K, device=DEV, generator=g).bfloat16()
     w = (torch.randn(N, K, device=DEV, generator=g) * K ** -0.5).bfloat16()
     ws = ops.dlinear_new_ws(ops.dlinear_ws_elems(N, K), device=DEV)
-    cnt = torch.zeros((N + 63) // 64, device=DEV, dtype=torch.int32)
+    cnt = torch.zeros((N + 63) // 64 + 1, device=DEV, dtype=torch.int32)  # + the ticket of the ssq_out sum
     ref = x.float() @ w.float().t()
     # (a) fp32 output, fused RMSNorm scale
     ssq = torch.zeros(16, device=DEV)
@@ -298,6 +298,11 @@ def test_dlinear(B, N, K, sched):
     close(xres, want)
     close(xg, xres.float() * gam, 1e-2)
     close(sso[:B], xres.float().pow(2).sum(-1), 1e-3)
+    # the sums of squares are added up in a fixed order: the same launch again gives the same bits
+    xres2, sso2 = res.clone(), torch.zeros(16, device=DEV)
+    ops.dlinear(x, w, xres2, ws=ws, counters=cnt, residual=xres2, gamma_next=gam, xg=xg, ssq_out=sso2, ssq_zero=ssz, sched=sched)
+    assert torch.equal(sso2, sso) and torch.equal(xres2, xres)
+    assert cnt.abs().max().item() == 0 and bool((ws.view(torch.int32) == -1).all())
     assert ssz.abs().max().item() == 0
     # (c) silu pair on interleaved rows
     if N % 2 == 0:
@@ -471,7 +476,7 @@ def test_topk_rows(T, K):
 
 @pytest.mark.parametrize("Sq,Sk", [(2049, 2049), (128, 128), (300, 77), (1, 1), (130, 257)])
 def test_flash_attention_d64(Sq, Sk):
-    """Fused tcgen05 attention (ViT head_dim 64) vs fp32 torch on the same bf16 q/k/v, incl. ragged tails."""
+    """Fused wgmma attention (ViT head_dim 64) vs fp32 torch on the same bf16 q/k/v, incl. ragged tails."""
     from u2tokenizer_b200 import ops
     B, H, dh = 2, 3, 64
     g = gen(Sq * 3 + Sk)
@@ -531,7 +536,7 @@ def test_sampling_distribution(temperature, top_k, top_p):
 
 @pytest.mark.parametrize("image,hidden,frames", [([8, 128, 256], 96, 3), ([32, 256, 256], 768, 5)])
 def test_patch_embed_fused(image, hidden, frames):
-    """One-kernel patch embedding (5-D TMA slabs -> converted A operand -> tcgen05, + bias + position table) against the
+    """One-kernel patch embedding (5-D TMA slabs -> converted A operand -> wgmma, + bias + position table) against the
     MONAI restatement in the oracle and against the unfused gather + GEMM path, canonical 4 x 16 x 16 patches."""
     from oracle import u2_oracle as O
     from u2tokenizer_b200 import ops

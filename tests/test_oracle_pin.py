@@ -1,8 +1,8 @@
-"""Pin the oracle (oracle/u2_oracle.py) against the REFERENCE modules imported unmodified from
-/root/reference, and the decoder restatement against the installed HF transformers models.
+"""Pin the oracle (oracle/u2_oracle.py) against the REFERENCE modules imported unmodified from the reference
+project, and the decoder restatement against the installed HF transformers models.
 
-Runs only where the reference tree is mounted (the authoring container); elsewhere the committed
-golden fixtures (tests/test_golden.py) carry the same pin."""
+Where the reference tree is not mounted the reference side comes from its recorded outputs (tests/golden/pins,
+see tests/refshim.py); the large SVR outputs are recorded as a fixed sample of their token rows."""
 import math
 
 import pytest
@@ -12,52 +12,59 @@ from common import fp32_sd, rel_err, tiny_geometry
 from oracle import u2_oracle as O
 import refshim
 
-needs_ref = pytest.mark.skipif(not refshim.have_reference(), reason="reference tree not mounted")
 TOL = 2e-5
+SVR_ROWS = torch.randperm(1792, generator=torch.Generator().manual_seed(0))[:128].sort().values  # recorded rows of (1, 1792, 512)
 
 
 def _sub(sd, prefix):
     return {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
 
 
-@needs_ref
 @pytest.mark.parametrize("attn_type", ["rma", "rope", "mha"])  # "mha": any other string -> nn.MultiheadAttention
 @pytest.mark.parametrize("diffts,dmtp,multi", [(True, True, True), (False, False, True), (True, False, False)])
 def test_u2tokenizer_matches_reference(attn_type, diffts, dmtp, multi):
-    refshim.install()
-    from src.model.u2tokenizer.u2Tokenizer import u2Tokenizer
     g = tiny_geometry(attn_type=attn_type, enable_diffts=diffts, enable_dmtp=dmtp, use_multi_scale=multi)
     sd = fp32_sd(g, seed=3)
-    ref = u2Tokenizer(embed_size=g.hidden_size, num_heads=g.u2t_num_heads, num_layers=g.u2t_num_layers,
-                      top_k=g.u2t_top_k, use_multi_scale=multi, num_3d_query_token=g.num_3d_query_token,
-                      hidden_size=g.hidden_size, attn_type=attn_type, enable_diffts=diffts, enable_dmtp=dmtp)
-    missing, unexpected = ref.load_state_dict(_sub(sd, "model.u2tokenizer."), strict=True)
     torch.manual_seed(0)
     v = torch.randn(2, 3, g.tokens_per_frame, g.hidden_size)
     t = torch.randn(2, 5, g.hidden_size)
+
+    def reference():
+        refshim.install()
+        from src.model.u2tokenizer.u2Tokenizer import u2Tokenizer
+        ref = u2Tokenizer(embed_size=g.hidden_size, num_heads=g.u2t_num_heads, num_layers=g.u2t_num_layers,
+                          top_k=g.u2t_top_k, use_multi_scale=multi, num_3d_query_token=g.num_3d_query_token,
+                          hidden_size=g.hidden_size, attn_type=attn_type, enable_diffts=diffts, enable_dmtp=dmtp)
+        ref.load_state_dict(_sub(sd, "model.u2tokenizer."), strict=True)
+        with torch.no_grad():
+            return ref(v_token=v, t_token=t)
+    want, _ = refshim.pinned(f"u2tokenizer_{attn_type}_{int(diffts)}{int(dmtp)}{int(multi)}", reference)
     with torch.no_grad():
-        want = ref(v_token=v, t_token=t)
         got = O.u2tokenizer(sd, "model.u2tokenizer.", v, t, g)
     assert got.shape == want.shape
     assert rel_err(got, want) < TOL
 
 
-@needs_ref
 @pytest.mark.parametrize("ptype", ["spatial", "sequence"])
 def test_projector_matches_reference(ptype):
-    refshim.install()
-    from src.model.multimodal_projector.spatial_pooling_projector import SpatialPoolingProjector
     g = tiny_geometry(proj_pooling_type=ptype)
     sd = fp32_sd(g, seed=4)
-    ref = SpatialPoolingProjector(image_size=g.image_size, patch_size=g.patch_size, in_dim=g.vit_hidden,
-                                  out_dim=g.hidden_size, layer_type=g.proj_layer_type, layer_num=g.proj_layer_num,
-                                  pooling_type=ptype, pooling_size=g.proj_pooling_size)
-    ref.load_state_dict(_sub(sd, "model.mm_projector."), strict=True)
-    x = torch.randn(3, g.n_patches, g.vit_hidden)
+    x = torch.randn(3, g.n_patches, g.vit_hidden, generator=torch.Generator().manual_seed(4))
+
+    def reference():
+        refshim.install()
+        from src.model.multimodal_projector.spatial_pooling_projector import SpatialPoolingProjector
+        ref = SpatialPoolingProjector(image_size=g.image_size, patch_size=g.patch_size, in_dim=g.vit_hidden,
+                                      out_dim=g.hidden_size, layer_type=g.proj_layer_type, layer_num=g.proj_layer_num,
+                                      pooling_type=ptype, pooling_size=g.proj_pooling_size)
+        ref.load_state_dict(_sub(sd, "model.mm_projector."), strict=True)
+        with torch.no_grad():
+            return {"out": ref(x), "proj_out_num": ref.proj_out_num}
+    pin, _ = refshim.pinned(f"projector_{ptype}", reference)
+    want = pin["out"]
     with torch.no_grad():
-        want = ref(x)
         got = O.spatial_pooling_projector(sd, "model.mm_projector.", x, g)
-    assert ref.proj_out_num == g.tokens_per_frame or ptype == "sequence"
+    assert pin["proj_out_num"] == g.tokens_per_frame or ptype == "sequence"
     assert rel_err(got, want) < TOL
 
 
@@ -69,53 +76,56 @@ def _hf_cfg_kwargs(g):
                 tie_word_embeddings=g.tie_word_embeddings, attention_bias=False)
 
 
-@needs_ref
 def test_full_model_matches_reference_llama():
     """forward() logits and greedy generate() ids of the reference u2LlamaForCausalLM (with the
     MONAI stand-in) equal the oracle's: pins the splice, the generate contract and the wiring."""
-    refshim.install()
-    from src.model.language_model.u2llama import u2Config, u2LlamaForCausalLM
-    from u2tokenizer_b200.configuration import MM_DEFAULTS
     rs = dict(factor=32.0, high_freq_factor=4.0, low_freq_factor=1.0,
               original_max_position_embeddings=64, rope_type="llama3")
     g = tiny_geometry(qk_norm=False, rope_theta=500000.0, rope_scaling=rs, rms_norm_eps=1e-5)
-    cfg = u2Config(**_hf_cfg_kwargs(g), rope_parameters=dict(rope_theta=g.rope_theta, **rs))
-    for k, v in MM_DEFAULTS.items():
-        setattr(cfg, k, v)
-    cfg.image_size, cfg.patch_size = g.image_size, g.patch_size
-    cfg.u2t_num_layers, cfg.u2t_top_k, cfg.num_3d_query_token = g.u2t_num_layers, g.u2t_top_k, g.num_3d_query_token
-    cfg.mm_hidden_size = g.vit_hidden
-    cfg.pretraining_tp = 1
-    torch.manual_seed(0)
-    import src.model.multimodal_encoder.vit as refvit
-    # the reference builds ViT-B/12 from MONAI defaults; shrink it through the same constructor args
-    orig = refvit.ViT.__init__
-
-    def small_init(self, *a, **kw):
-        kw.update(hidden_size=g.vit_hidden, mlp_dim=g.vit_mlp, num_layers=g.vit_layers, num_heads=g.vit_heads)
-        orig(self, *a, **kw)
-    refvit.ViT.__init__ = small_init
-    try:
-        model = u2LlamaForCausalLM(cfg)
-        from src.model.u2tokenizer.builder import build_u2tokenizer_tower
-        model.get_model().u2tokenizer = build_u2tokenizer_tower(cfg)
-    finally:
-        refvit.ViT.__init__ = orig
     sd = fp32_sd(g, seed=5)
-    res = model.load_state_dict(sd, strict=False)
-    assert not res.unexpected_keys, res.unexpected_keys
-    assert all("rotary" in k or "inv_freq" in k for k in res.missing_keys), res.missing_keys
-    model.eval().float()
     from u2tokenizer_b200.synthetic import synthetic_inputs
     images, ids, qids = synthetic_inputs(g, batch=2, frames=2, n_question=6, lt=12, im_patch_id=g.vocab_size - 2)
+
+    def reference():
+        refshim.install()
+        from src.model.language_model.u2llama import u2Config, u2LlamaForCausalLM
+        from u2tokenizer_b200.configuration import MM_DEFAULTS
+        cfg = u2Config(**_hf_cfg_kwargs(g), rope_parameters=dict(rope_theta=g.rope_theta, **rs))
+        for k, v in MM_DEFAULTS.items():
+            setattr(cfg, k, v)
+        cfg.image_size, cfg.patch_size = g.image_size, g.patch_size
+        cfg.u2t_num_layers, cfg.u2t_top_k, cfg.num_3d_query_token = g.u2t_num_layers, g.u2t_top_k, g.num_3d_query_token
+        cfg.mm_hidden_size = g.vit_hidden
+        cfg.pretraining_tp = 1
+        torch.manual_seed(0)
+        import src.model.multimodal_encoder.vit as refvit
+        # the reference builds ViT-B/12 from MONAI defaults; shrink it through the same constructor args
+        orig = refvit.ViT.__init__
+
+        def small_init(self, *a, **kw):
+            kw.update(hidden_size=g.vit_hidden, mlp_dim=g.vit_mlp, num_layers=g.vit_layers, num_heads=g.vit_heads)
+            orig(self, *a, **kw)
+        refvit.ViT.__init__ = small_init
+        try:
+            model = u2LlamaForCausalLM(cfg)
+            from src.model.u2tokenizer.builder import build_u2tokenizer_tower
+            model.get_model().u2tokenizer = build_u2tokenizer_tower(cfg)
+        finally:
+            refvit.ViT.__init__ = orig
+        res = model.load_state_dict(sd, strict=False)
+        assert not res.unexpected_keys, res.unexpected_keys
+        assert all("rotary" in k or "inv_freq" in k for k in res.missing_keys), res.missing_keys
+        model.eval().float()
+        with torch.no_grad():
+            logits = model(images=images, input_ids=ids, question_ids=qids).logits
+            gen_ids = model.generate(images, ids, question_ids=qids, max_new_tokens=6, do_sample=False)
+        return {"logits": logits, "ids": gen_ids[:, -6:]}
+    want, _ = refshim.pinned("full_model_llama", reference)
     with torch.no_grad():
-        want = model(images=images, input_ids=ids, question_ids=qids).logits
         got = O.forward_logits(sd, ids, images, qids, g)
-        assert rel_err(got, want) < 1e-4
-        want_ids = model.generate(images, ids, question_ids=qids, max_new_tokens=6, do_sample=False)
+        assert rel_err(got, want["logits"]) < 1e-4
         got_ids, margins = O.greedy_generate(sd, ids, images, qids, g, max_new_tokens=6)
-    assert torch.equal(got_ids, want_ids[:, -6:]) or bool((margins.min() < 1e-4))
-    assert torch.equal(got_ids, want_ids[:, -6:])
+    assert torch.equal(got_ids, want["ids"])
 
 
 @pytest.mark.parametrize("family", ["qwen3", "llama"])
@@ -152,46 +162,56 @@ def test_decoder_matches_hf(family):
 # ------------------------------------------------------------------------------------------------
 # the reference's own two smoke runs (the only "known answers" it holds, SURVEY.md section 4)
 # ------------------------------------------------------------------------------------------------
-@needs_ref
 @pytest.mark.parametrize("diffts,dmtp", [(False, False), (True, True)])
 def test_reference_smoke_run_svr(diffts, dmtp):
     """src/model/u2tokenizer/svr.py:190-205: SpatioTemporalVisualTokenRefinerModel(512, 8 heads, 4 layers, top_k 1024,
     multi-scale, "rope") on [1, 64, 256, 512] prints (1, 1792, 512). (False, False) is that block's own configuration,
     (True, True) the canonical DiffTS + DMTP one."""
-    refshim.install()
-    from src.model.u2tokenizer.svr import SpatioTemporalVisualTokenRefinerModel
     g = tiny_geometry(hidden_size=512, attn_type="rope", u2t_num_heads=8, u2t_num_layers=4, u2t_top_k=1024,
                       use_multi_scale=True, enable_diffts=diffts, enable_dmtp=dmtp)
     sd = fp32_sd(g, seed=11)
-    ref = SpatioTemporalVisualTokenRefinerModel(embed_size=512, num_heads=8, num_layers=4, top_k=1024, use_multi_scale=True,
-                                                attn_type="rope", enable_diffts=diffts, enable_dmtp=dmtp)
-    ref.load_state_dict(_sub(sd, "model.u2tokenizer.svt_module."), strict=True)
     x = torch.randn(1, 64, 256, 512, generator=torch.Generator().manual_seed(5))
+
+    def reference():
+        refshim.install()
+        from src.model.u2tokenizer.svr import SpatioTemporalVisualTokenRefinerModel
+        ref = SpatioTemporalVisualTokenRefinerModel(embed_size=512, num_heads=8, num_layers=4, top_k=1024, use_multi_scale=True,
+                                                    attn_type="rope", enable_diffts=diffts, enable_dmtp=dmtp)
+        ref.load_state_dict(_sub(sd, "model.u2tokenizer.svt_module."), strict=True)
+        with torch.no_grad():
+            return {"shape": tuple(ref(x).shape), "out": ref(x)}
+    pin, full = refshim.pinned(f"svr_smoke_{int(diffts)}{int(dmtp)}", reference,
+                               keep=lambda p: {"shape": p["shape"], "out": p["out"][:, SVR_ROWS].clone()})
+    want = pin["out"]
     with torch.no_grad():
-        want = ref(x)
         got = O.svr(sd, "model.u2tokenizer.svt_module.", x, g)
-    assert tuple(want.shape) == (1, 1792, 512) == tuple(got.shape)     # the shape the reference prints
+    assert tuple(pin["shape"]) == (1, 1792, 512) == tuple(got.shape)     # the shape the reference prints
+    if not full:
+        got = got[:, SVR_ROWS]
     # hard selection over 16384 near-identical scores is decided by the last float bits: the selected SET may differ
     # between two fp32 evaluations, the selected VALUES (and everything downstream) may not
     assert rel_err(got, want) < (TOL if diffts else 1e-3)
 
 
-@needs_ref
 def test_reference_smoke_run_tta():
     """src/model/u2tokenizer/tta.py:142-151: TextConditionTokenAggregatorModel(896, 4 layers, 8 heads, "rope") on query
     [1, 64, 896], visual [1, 1792, 896], text [1, 755, 896] prints (1, 64, 896)."""
-    refshim.install()
-    from src.model.u2tokenizer.tta import TextConditionTokenAggregatorModel
     g = tiny_geometry(hidden_size=896, attn_type="rope", u2t_num_heads=8, u2t_num_layers=4)
     sd = fp32_sd(g, seed=12)
-    ref = TextConditionTokenAggregatorModel(896, 4, 8, attn_type="rope")
-    ref.load_state_dict(_sub(sd, "model.u2tokenizer.tta_module."), strict=True)
     gen = torch.Generator().manual_seed(6)
     q = torch.randn(1, 64, 896, generator=gen)
     vis = torch.randn(1, 1792, 896, generator=gen)
     txt = torch.randn(1, 755, 896, generator=gen)
+
+    def reference():
+        refshim.install()
+        from src.model.u2tokenizer.tta import TextConditionTokenAggregatorModel
+        ref = TextConditionTokenAggregatorModel(896, 4, 8, attn_type="rope")
+        ref.load_state_dict(_sub(sd, "model.u2tokenizer.tta_module."), strict=True)
+        with torch.no_grad():
+            return ref(q, vis, txt)
+    want, _ = refshim.pinned("tta_smoke", reference)
     with torch.no_grad():
-        want = ref(q, vis, txt)
         got = O.tta(sd, "model.u2tokenizer.tta_module.", q, vis, txt, g)
     assert tuple(want.shape) == (1, 64, 896) == tuple(got.shape)       # the shape the reference prints
     assert rel_err(got, want) < TOL

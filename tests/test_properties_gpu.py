@@ -62,7 +62,7 @@ def test_cross_attention_identical_keys_gives_value_mean():
 
 
 def test_decode_equals_teacher_forced_prefill_full_width():
-    """Qwen3-8B widths (E 4096, 32/8 heads of 128, I 12288): KV-cached decode steps on the tcgen05 stream-K path
+    """Qwen3-8B widths (E 4096, 32/8 heads of 128, I 12288): KV-cached decode steps on the wgmma stream-K path
     reproduce the teacher-forced prefill logits of the same tokens (both paths share only the weights)."""
     eng, g = _engine()
     B, L = 4, 40
@@ -85,7 +85,7 @@ def test_decode_equals_teacher_forced_prefill_full_width():
 
 def test_vit_attention_permutation_equivariance():
     """Non-causal attention without positional bias is equivariant to a permutation of the keys/values and
-    the fused tcgen05 kernel must agree with the unfused GEMM -> softmax -> GEMM path (S = 2049)."""
+    the fused wgmma kernel must agree with the unfused GEMM -> softmax -> GEMM path (S = 2049)."""
     eng, g = _engine()
     F_, S, H, dh = 2, 2049, 12, 64
     Sp = (S + 7) // 8 * 8

@@ -414,7 +414,7 @@ CASES = {
     "hard_selection_plain_pool": dict(enable_diffts=False, enable_dmtp=False, u2t_top_k=8),
     "llama_tied": dict(qk_norm=False, tie_word_embeddings=True, head_dim=32, rope_theta=500000.0),
     "sequence_pool_no_multiscale": dict(proj_pooling_type="sequence", use_multi_scale=False),
-    # ViT head_dim 64: fused tcgen05 attention forward + probabilities recomputed in the backward (the production ViT-B path)
+    # ViT head_dim 64: fused wgmma attention forward + probabilities recomputed in the backward (the production ViT-B path)
     "vit_head_dim_64_flash_recompute": dict(vit_hidden=128, vit_heads=2, vit_mlp=256),
 }
 

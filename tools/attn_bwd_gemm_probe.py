@@ -43,4 +43,4 @@ for name, fn in runs.items():
     ms = e0.elapsed_time(e1) / reps
     tiles = b * h * ((S + 127) // 128) * ((S + 255) // 256)
     print(f"{name:20s} {ms * 1e3:8.1f} us  {fl / ms / 1e9:6.0f} TFLOP/s  {b * h * S * Sp * 2 / ms / 1e6:6.0f} GB/s written  "
-          f"{ms * 1e3 / (tiles / 148):.2f} us per tile and SM", flush=True)
+          f"{ms * 1e3 / (tiles / 132):.2f} us per tile and SM", flush=True)

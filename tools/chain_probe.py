@@ -17,7 +17,7 @@ gridbar = torch.zeros(4 * nlay, device=dev, dtype=torch.int32); step = torch.zer
 ssq_a, ssq_b = torch.zeros(16, device=dev), torch.zeros(16, device=dev)
 x = rnd(B, E).bfloat16(); xg = torch.empty_like(x); xg2 = torch.empty_like(x); ctx = rnd(B, E).bfloat16()
 act = torch.empty(B, I, device=dev, dtype=torch.bfloat16); qkv = torch.empty(B, NQ, device=dev, dtype=torch.bfloat16)
-dbg = torch.zeros(148 * 4 * 8, device=dev, dtype=torch.int64)
+dbg = torch.zeros(132 * 4 * 8, device=dev, dtype=torch.int64)
 def chain(l, d=None):
     w = W[l]
     sc = int(os.environ.get("U2_DL_SCHED", "0"))
@@ -45,7 +45,7 @@ e1.record(); torch.cuda.synchronize()
 print(f"chain launch: {e0.elapsed_time(e1) * 1e3 / nlay:.1f} us each (stream-only bound {2 * (E * E + 2 * I * E + E * I + NQ * E) / 6.4e6:.1f} us)")
 step += 1
 ops.dlinear_multi(chain(2, dbg), gridbar=gridbar[8:12], step_dev=step, lookahead_units=LA, next_weights=nxw(2), pre_stages=int(os.environ.get("U2_PRE_STAGES", "0"))); torch.cuda.synchronize()
-d = dbg.view(148, 4, 8).cpu()
+d = dbg.view(132, 4, 8).cpu()
 t0 = d[:, 0, 0].min().item()
 rel = (d - t0).float() / 1e3
 names = ["Wpre", "dep ok", "1st full", "last commit", "last acc", "epi done", "fin wait", "fin got"]

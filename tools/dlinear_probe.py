@@ -8,7 +8,7 @@ def probe(N, K, reps=40, nw=24, pdl=True):
     x = torch.randn(B, K, device="cuda").bfloat16()
     W = [(torch.randn(N, K, device="cuda") * 0.02).bfloat16() for _ in range(nw)]
     out = torch.empty(B, N, device="cuda", dtype=torch.bfloat16)
-    dbg = torch.zeros(148 * 8, device="cuda", dtype=torch.int64)
+    dbg = torch.zeros(132 * 8, device="cuda", dtype=torch.int64)
     for w in W: ops.dlinear(x, w, out, ws=ws, counters=cnt, pdl=pdl)
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -18,7 +18,7 @@ def probe(N, K, reps=40, nw=24, pdl=True):
     e1.record(); torch.cuda.synchronize()
     us = e0.elapsed_time(e1) * 1e3 / reps
     torch.cuda.synchronize()
-    d = dbg.view(148, 8).cpu()
+    d = dbg.view(132, 8).cpu()
     t0 = d[:, 0].min().item()
     rel = (d - t0).float() / 1e3
     names = ["entry", "setup", "x-wait", "1st full", "last commit", "epi got", "epi done", "exit"]

@@ -1,4 +1,4 @@
-"""u2tokenizer_b200: a B200-native (sm_100a) implementation of the mu2-LLM hot path.
+"""u2tokenizer_b200: a H100-native (sm_90a) implementation of the mu2-LLM hot path.
 
 CT volume -> 3D patch embedding -> ViT3D -> spatial-pooling projector -> mu2-Tokenizer ->
 splice into the prompt embeddings -> Qwen3/Llama decoder forward / greedy generate.

@@ -207,6 +207,7 @@ SIGNATURES = {
     "u2_transpose_heads_bf16": (C.c_int, [_P, _P, _I, _I, _I, _I, _L, _L, _L, _L, _L, _L, _P]),
     "u2_spp_pool_bf16": (C.c_int, [_P, _P, _L, _I, _I, _I, _I, _I, _L, _L, _L, _I, _P]),
     "u2_multiscale_pool_bf16": (C.c_int, [_P, _P, _P, _F, _P, _I, _I, _I, _I, _P]),
+    "u2_multiscale_pool_ws_elems": (C.c_int64, [_I, _I]),
     "u2_embed_splice_bf16": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _L, _P]),
     "u2_temporal_attention_bf16": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _L, _L, _F, _P, _I, _P]),
     "u2_rope_bf16": (C.c_int, [_P, C.POINTER(RopeDesc), _P]),
@@ -278,8 +279,8 @@ def load():
     return lib
 
 
-# kernels launched per entry point (u2_multiscale_pool_bf16: gate + write, counted at its maximum)
-KERNELS_PER_CALL = {"u2_multiscale_pool_bf16": 2, "u2_argmax_f32": 2, "u2_lmhead_logprob_bf16": 2,
+# kernels launched per entry point (u2_multiscale_pool_bf16: gate + gate sum + write, counted at its maximum)
+KERNELS_PER_CALL = {"u2_multiscale_pool_bf16": 3, "u2_argmax_f32": 2, "u2_lmhead_logprob_bf16": 2,
                     "u2_preprocess_volume_f32": 14, "u2_multiscale_pool_bwd_bf16": 2}
 _launches = 0
 

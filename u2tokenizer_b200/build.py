@@ -1,4 +1,4 @@
-"""Build libu2b200.so (the sm_100a kernels + C ABI) in-tree with nvcc.
+"""Build libu2b200.so (the sm_90a kernels + C ABI) in-tree with nvcc.
 
 No JIT cache, no torch extension machinery: plain ``nvcc -c`` per translation unit (in parallel)
 and one ``nvcc -shared`` link, output next to this file so it travels with the source tree.
@@ -20,7 +20,7 @@ LIB_PATH = PKG_DIR / "libu2b200.so"
 BUILD_DIR = REPO / "build" / "obj"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     "--expt-relaxed-constexpr",
@@ -75,7 +75,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     need_link = force or bool(jobs) or not LIB_PATH.exists() or any(
         o.stat().st_mtime > LIB_PATH.stat().st_mtime for o in objs)
     if need_link:
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static",
+        cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static",
                "-o", str(LIB_PATH), *map(str, objs)]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

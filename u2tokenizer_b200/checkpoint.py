@@ -6,7 +6,7 @@ pointing at two python files stored next to the weights
 ``modeling_u2Llama.u2LlamaForCausalLM``) and loads them with
 ``AutoModelForCausalLM.from_pretrained(path, trust_remote_code=True)`` (src/train/train_stage2.py:145-152,
 eval/mrg.py:42-45). The state-dict keys of those classes are the ones ``modeling.py`` reproduces, so switching a
-checkpoint directory to the B200 path means replacing the two python files by thin shims that re-export the classes of
+checkpoint directory to the H100 path means replacing the two python files by thin shims that re-export the classes of
 this package under the reference's file and class names; the weights, tokenizer files and ``config.json`` stay as
 they are. ``write_remote_code`` does exactly that; ``save_pretrained`` writes a complete directory from a model.
 """
@@ -22,7 +22,7 @@ _FAMILIES = {
 }
 _CONFIG_STEM, _CONFIG_CLASS = "configuration_u2", "u2Config"
 
-_CONFIG_SHIM = '''"""Remote-code shim: the configuration class of the B200 path under the reference's name
+_CONFIG_SHIM = '''"""Remote-code shim: the configuration class of the H100 path under the reference's name
 (replaces the reference's configuration_u2.py in a checkpoint directory)."""
 from u2tokenizer_b200.configuration import {cfg} as _Base
 
@@ -31,7 +31,7 @@ class u2Config(_Base):
     pass
 '''
 
-_MODEL_SHIM = '''"""Remote-code shim: the B200 implementation under the reference's module / class name
+_MODEL_SHIM = '''"""Remote-code shim: the H100 implementation under the reference's module / class name
 (replaces the reference's {stem}.py in a checkpoint directory; same state-dict keys, same forward / generate)."""
 from u2tokenizer_b200.modeling import {pkg_cls} as _Base
 

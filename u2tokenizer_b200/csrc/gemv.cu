@@ -228,11 +228,11 @@ template <int kB>
 static int launch_gemv(const GemvArgs& a, cudaStream_t st) {
   const int n_out = a.silu_pair ? a.N / 2 : a.N;
   const int wpb = 4;
-  // 4 rows per warp when there are plenty of rows, else 2 / 1 so that the grid still fills 148 SMs
-  if (!a.silu_pair && n_out >= 148 * 4 * wpb * 4) {
+  // 4 rows per warp when there are plenty of rows, else 2 / 1 so that the grid still fills 132 SMs
+  if (!a.silu_pair && n_out >= 132 * 4 * wpb * 4) {
     const int rpb = wpb * 4;
     gemv_kernel<kB, 4><<<(n_out + rpb - 1) / rpb, wpb * 32, 0, st>>>(a);
-  } else if (n_out >= 148 * 2 * wpb * 2) {
+  } else if (n_out >= 132 * 2 * wpb * 2) {
     const int rpb = wpb * 2;
     gemv_kernel<kB, 2><<<(n_out + rpb - 1) / rpb, wpb * 32, 0, st>>>(a);
   } else {

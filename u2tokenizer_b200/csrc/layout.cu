@@ -235,11 +235,13 @@ seq_pool_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__
 
 // ------------------------------------------------------------------------------------------------
 // multi-scale pooling (scales 1, 2, 4 over the token dim) with the dynamic gate:
-//   pass 1 (gate): logits[b][k] += sum_e w[e] * mean_tokens(pool_k(x))[e]   (atomics, 3 per block)
+//   pass 1 (gate): part[b][blk][k] = sum over the block's rows of sum_e w[e] * pool_k(x)[e] / covered rows
+//   pass 1b:       logits[b][k] = sum_blk part[b][blk][k], in block order (the same bits on every run; float
+//                  atomics would add the blocks in the order they happen to finish)
 //   pass 2 (write): out[b] = cat_k softmax(logits[b] + bias)[k] * pool_k(x[b])
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-msp_gate_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gate_w, float* __restrict__ logits,
+msp_gate_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gate_w, float* __restrict__ part,
                 int K, int E, int rows_per_block) {
   // grid: (ceil(K / rows_per_block), B); each thread owns E/8-vector columns strided by blockDim
   const int b = blockIdx.y;
@@ -281,7 +283,17 @@ msp_gate_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ g
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += red[threadIdx.x][w];
     // mean over the pooled tokens of scale k == sum over the covered input rows / covered rows
     const int denom = threadIdx.x == 0 ? K : (threadIdx.x == 1 ? n2 : n4);
-    if (denom > 0) atomicAdd(&logits[b * 3 + threadIdx.x], s / denom);
+    part[((long long)b * gridDim.x + blockIdx.x) * 3 + threadIdx.x] = denom > 0 ? s / denom : 0.f;
+  }
+}
+
+__global__ void __launch_bounds__(256)
+msp_gate_sum_kernel(const float* __restrict__ part, float* __restrict__ logits, int B, int nblk) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 3 * B; i += gridDim.x * blockDim.x) {
+    const int b = i / 3, k = i - 3 * b;
+    float s = 0.f;
+    for (int j = 0; j < nblk; ++j) s += part[((long long)b * nblk + j) * 3 + k];
+    logits[i] = s;
   }
 }
 
@@ -357,7 +369,7 @@ embed_splice_kernel(const long long* __restrict__ ids, const __nv_bfloat16* __re
 
 static inline unsigned grid_for(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
-  const long long cap = 148LL * 32;
+  const long long cap = 132LL * 32;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
   return (unsigned)b;
@@ -452,6 +464,13 @@ extern "C" U2_API int u2_spp_pool_bf16(const void* x, void* out, int64_t frames,
   return U2_OK;
 }
 
+constexpr int kMspRowsPerBlock = 16;
+
+extern "C" U2_API int64_t u2_multiscale_pool_ws_elems(int32_t B, int32_t K) {
+  if (B <= 0 || K <= 0) return 0;
+  return 3LL * B * (1 + (K + kMspRowsPerBlock - 1) / kMspRowsPerBlock);
+}
+
 extern "C" U2_API int u2_multiscale_pool_bf16(const void* x, void* out, const float* gate_w, float gate_bias,
                                               float* logits_ws, int32_t B, int32_t K, int32_t E, int32_t dynamic,
                                               void* stream) {
@@ -459,13 +478,15 @@ extern "C" U2_API int u2_multiscale_pool_bf16(const void* x, void* out, const fl
   if (E & 7) return set_error(U2_ERR_ARG, "multiscale_pool: E must be a multiple of 8");
   if (B <= 0 || K <= 0) return U2_OK;
   if (dynamic) {
-    if (!gate_w || !logits_ws) return set_error(U2_ERR_ARG, "multiscale_pool: dynamic gate needs gate_w and a [B,3] fp32 workspace");
-    cudaError_t e = cudaMemsetAsync(logits_ws, 0, sizeof(float) * 3 * B, ST(stream));
-    if (e != cudaSuccess) return set_error(U2_ERR_CUDA, "multiscale_pool memset: %s", cudaGetErrorString(e));
-    const int rpb = 16;
-    dim3 grid((unsigned)((K + rpb - 1) / rpb), (unsigned)B);
-    msp_gate_kernel<<<grid, 256, 0, ST(stream)>>>(CBF(x), gate_w, logits_ws, K, E, rpb);
+    if (!gate_w || !logits_ws)
+      return set_error(U2_ERR_ARG, "multiscale_pool: dynamic gate needs gate_w and a u2_multiscale_pool_ws_elems(B, K) fp32 workspace");
+    const int nblk = (K + kMspRowsPerBlock - 1) / kMspRowsPerBlock;
+    float* part = logits_ws + 3 * B;
+    dim3 grid((unsigned)nblk, (unsigned)B);
+    msp_gate_kernel<<<grid, 256, 0, ST(stream)>>>(CBF(x), gate_w, part, K, E, kMspRowsPerBlock);
     U2_CHECK_LAUNCH("multiscale_pool gate");
+    msp_gate_sum_kernel<<<(unsigned)((3 * B + 255) / 256), 256, 0, ST(stream)>>>(part, logits_ws, B, nblk);
+    U2_CHECK_LAUNCH("multiscale_pool gate sum");
   }
   const int n_out = K + (K >= 2 ? K / 2 : 0) + (K >= 4 ? K / 4 : 0);
   const long long total = (long long)B * n_out * (E / 8);

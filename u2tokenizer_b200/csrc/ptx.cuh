@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a primitives the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and fences.
+// Thin inline-PTX wrappers for the sm_90a primitives the kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA) and fences.
 // Everything here is device-side and header-only.
 #pragma once
 #include <cuda_runtime.h>
@@ -140,115 +140,73 @@ __device__ __forceinline__ void sts64(uint32_t addr, uint32_t lo, uint32_t hi) {
   asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(lo), "r"(hi) : "memory");
 }
 
-// generic-proxy writes to smem -> visible to the async proxy (TMA store / UMMA operand reads)
+// generic-proxy writes to smem -> visible to the async proxy (TMA store / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (sm_90a warpgroup MMA): bf16 x bf16 -> fp32, accumulators in registers
 // ----------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "power of two in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
 
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16/f16 inputs, fp32 accumulate, single CTA.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}"
-      :
-      : "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// All previously issued tcgen05.mma of this thread arrive (once) on the mbarrier when complete.
-// Implies tcgen05.fence::before_thread_sync.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes (lane quarter = warp_id % 4), 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// UMMA descriptors (sm_100 "version 1" shared-memory matrix descriptor, instruction descriptor)
-// ----------------------------------------------------------------------------------------------
-// K-major operand tile stored as rows of 128 bytes (64 bf16) with the 128-byte TMA/UMMA swizzle:
-// 8-row groups are 1024 B apart (stride byte offset); the leading offset is unused for this mode.
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);  // start address, bits [0,14)
-  d |= static_cast<uint64_t>(0) << 16;                      // leading byte offset (ignored)
-  d |= static_cast<uint64_t>(1024u >> 4) << 32;             // stride byte offset, bits [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                      // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                      // layout type: SWIZZLE_128B
-  return d;
-}
-
-// MN-major operand tile (the contraction index is the slow, row index of the stored matrix): 64-element (128-byte)
-// MN chunks of 8-row (k) groups, 128-byte swizzle. LBO = byte distance between consecutive 64-wide MN chunks,
-// SBO = 1024 B between consecutive groups of 8 k-rows.
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
+// Shared-memory matrix descriptor (sm_90) of a tile stored with the 128-byte TMA swizzle: 8-row (K-major) or 8-k-row
+// (MN-major) groups 1024 B apart (stride byte offset). For an MN-major tile the leading byte offset is the distance
+// between consecutive 64-element MN chunks; a K-major tile ignores it.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes = 16) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);  // start address, bits [0,14)
   d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;         // leading byte offset, bits [16,30)
   d |= static_cast<uint64_t>(1024u >> 4) << 32;             // stride byte offset, bits [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                      // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                      // layout type: SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                      // layout type: SWIZZLE_128B
   return d;
 }
 
-// kind::f16 instruction descriptor: bf16 x bf16 -> fp32, both operands K-major, M x N tile.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t m, uint32_t n) {
-  return (1u << 4)           // accumulator format: F32
-         | (1u << 7)         // A format: BF16
-         | (1u << 10)        // B format: BF16
-         | (0u << 15)        // A K-major
-         | (0u << 16)        // B K-major
-         | ((n >> 3) << 17)  // N / 8
-         | ((m >> 4) << 24); // M / 16
+// D (64 x 64, fp32 fragment) (+)= A (64 x 16, smem) * B (64 x 16, smem)^T. kTransA / kTransB: operand stored MN-major.
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(kTransA), "n"(kTransB));
 }
+
+// Same with A (64 x 16 bf16) taken from registers: a[0..3] is the m64k16 A fragment of this thread.
+template <int kTransB>
+__device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc) {
+  asm volatile(
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, 1, 1, 1, %37;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "n"(kTransB));
+}
+
+// D (64 x 16) (+)= A (64 x 16) * B (16 x 16)^T, both operands K-major in shared memory.
+__device__ __forceinline__ void wgmma_m64n16k16_ss(float (&d)[8], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
+// Accumulator fragment of an m64nN wgmma: element j of this thread (warp w of the warpgroup, lane l) holds
+//   row 16 w + l / 4 + 8 ((j >> 1) & 1),  column 8 (j >> 2) + 2 (l % 4) + (j & 1).
 
 }  // namespace u2

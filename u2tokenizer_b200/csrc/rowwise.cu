@@ -440,7 +440,7 @@ extern "C" U2_API int u2_silu_mul_bf16(const void* gate_up, void* out, int64_t r
   if (rows <= 0) return U2_OK;
   const long long total = rows * (I / 8);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 16) blocks = 148LL * 16;
+  if (blocks > 132LL * 16) blocks = 132LL * 16;
   silu_mul_kernel<<<(unsigned)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __nv_bfloat16*>(gate_up), reinterpret_cast<__nv_bfloat16*>(out), rows, I, ldg, ldo, interleaved);
   U2_CHECK_LAUNCH("silu_mul");

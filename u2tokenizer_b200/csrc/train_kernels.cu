@@ -1,6 +1,6 @@
 // Training-side kernels (everything of the backward pass that is not a GEMM): HBM-bound row-wise / elementwise
 // work, 16-byte vector accesses, fp32 statistics, fp32 accumulators for the small parameter gradients.
-// The contractions (dgrad, wgrad, dP, dQ, dK, dV) run on gemm_tcgen05.cu with its MN-major operand flags.
+// The contractions (dgrad, wgrad, dP, dQ, dK, dV) run on gemm_wgmma.cu with its MN-major operand flags.
 // Declared in include/u2b200_train.h; reference call sites: HF Trainer backward over the modules of src/model
 // (train_stage1.py:244-250), DeepSpeed ZeRO-1 optimizer step (config/ds_config.json:27-39).
 #include <cuda_bf16.h>
@@ -45,7 +45,7 @@ __device__ __forceinline__ void t_load8f(const float* p, float (&f)[8]) {
   const float4 a = reinterpret_cast<const float4*>(p)[0], b = reinterpret_cast<const float4*>(p)[1];
   f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
 }
-static inline unsigned t_grid(long long total, int threads, long long cap = 148LL * 16) {
+static inline unsigned t_grid(long long total, int threads, long long cap = 132LL * 16) {
   long long b = (total + threads - 1) / threads;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
@@ -285,7 +285,7 @@ static int launch_norm_bwd(const void* x, const float* gamma, const void* dy, co
   if (rows <= 0) return U2_OK;
   const int need = (E / 8 + 31) / 32;
   long long blocks = (rows + 7) / 8;
-  if (blocks > 148 * 2) blocks = 148 * 2;
+  if (blocks > 132 * 2) blocks = 132 * 2;
   const size_t smem = dgamma ? (size_t)(kRms ? E : 2 * E) * sizeof(float) : 0;
 #define U2_NB_CASE(MV)                                                                                                 \
   do {                                                                                                                 \
@@ -1092,7 +1092,7 @@ extern "C" U2_API int u2_colsum_bf16(const void* x, float* out, int64_t rows, in
   if (cols <= 0 || (cols & 7) || (ld & 7)) return set_error(U2_ERR_ARG, "colsum: cols / ld must be multiples of 8");
   if (rows <= 0) return U2_OK;
   const long long gx = (cols + 255) / 256;
-  long long gy = (148LL * 4 + gx - 1) / gx;
+  long long gy = (132LL * 4 + gx - 1) / gx;
   long long rpb = (rows + gy - 1) / gy;
   if (rpb < 64) rpb = 64;
   gy = (rows + rpb - 1) / rpb;
@@ -1202,7 +1202,7 @@ extern "C" U2_API int u2_rowdot_bf16(const void* a, const void* c, float* out, i
   if ((dh & 1) || ((a_sb | a_ss | a_sh | c_sb | c_ss | c_sh) & 1)) return set_error(U2_ERR_ARG, "rowdot: dh / strides must be even");
   if (B <= 0 || S <= 0 || H <= 0) return U2_OK;
   long long blocks = ((long long)B * S * H + 7) / 8;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   rowdot_kernel<<<(unsigned)blocks, 256, 0, ST(stream)>>>(CBF(a), CBF(c), out, B, S, H, dh, a_sb, a_ss, a_sh, c_sb, c_ss, c_sh);
   U2_CHECK_LAUNCH("rowdot");
   return U2_OK;
@@ -1249,7 +1249,7 @@ extern "C" U2_API int u2_rope_bwd_bf16(void* dx, const void* x_raw, const u2_rop
   a.dk_norm_w = d->k_norm_w ? dk_norm_w : nullptr;
   const long long items = d->rows * (long long)(a.n_q_heads + a.n_k_heads);
   long long blocks = (items + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   const size_t smem = (a.dq_norm_w || a.dk_norm_w) ? (size_t)2 * a.dh * sizeof(float) : 0;
   rope_bwd_kernel<<<(unsigned)blocks, 256, smem, ST(stream)>>>(a);
   U2_CHECK_LAUNCH("rope_bwd");
@@ -1262,7 +1262,7 @@ extern "C" U2_API int u2_spp_pool_bwd_bf16(const void* dy, void* dx, int64_t fra
   if (!dy || !dx) return set_error(U2_ERR_ARG, "spp_pool_bwd: null pointer");
   if ((E & 7) || (ldx & 7) || ps <= 0) return set_error(U2_ERR_ARG, "spp_pool_bwd: E / ldx must be multiples of 8");
   if (frames <= 0) return U2_OK;
-  spp_pool_bwd_kernel<<<t_grid(frames * rows_per_frame * (E / 8), 256, 148LL * 32), 256, 0, ST(stream)>>>(
+  spp_pool_bwd_kernel<<<t_grid(frames * rows_per_frame * (E / 8), 256, 132LL * 32), 256, 0, ST(stream)>>>(
       CBF(dy), BF(dx), frames, g0, g1, g2, ps, E, in_frame_stride, in_off, ldx, rows_per_frame, sequence);
   U2_CHECK_LAUNCH("spp_pool_bwd");
   return U2_OK;
@@ -1314,7 +1314,7 @@ extern "C" U2_API int u2_ce_bwd_f32_bf16(const float* logits, void* dlogits, con
   if (!logits || !dlogits || !lse || !labels || !coef) return set_error(U2_ERR_ARG, "ce_bwd: null pointer");
   if ((V & 7) || (ld_in & 3) || (ld_out & 7)) return set_error(U2_ERR_ARG, "ce_bwd: V / ld must be multiples of 8");
   if (R <= 0) return U2_OK;
-  ce_bwd_kernel<<<t_grid(R * (V / 8), 256, 148LL * 32), 256, 0, ST(stream)>>>(logits, BF(dlogits), lse,
+  ce_bwd_kernel<<<t_grid(R * (V / 8), 256, 132LL * 32), 256, 0, ST(stream)>>>(logits, BF(dlogits), lse,
                                                                             reinterpret_cast<const long long*>(labels), coef, R, V, ld_in, ld_out);
   U2_CHECK_LAUNCH("ce_bwd");
   return U2_OK;
@@ -1347,7 +1347,7 @@ extern "C" U2_API int u2_adamw_bf16(float* master, float* m, float* v, const voi
   int rc = adam_args(desc, &a);
   if (rc) return rc;
   if (n <= 0) return U2_OK;
-  adamw_kernel<false><<<t_grid(n / 4, 256, 148LL * 16), 256, 0, ST(stream)>>>(master, m, v, grad, BF(param_out), nullptr, n, a);
+  adamw_kernel<false><<<t_grid(n / 4, 256, 132LL * 16), 256, 0, ST(stream)>>>(master, m, v, grad, BF(param_out), nullptr, n, a);
   U2_CHECK_LAUNCH("adamw");
   return U2_OK;
 }
@@ -1360,7 +1360,7 @@ extern "C" U2_API int u2_adamw_bf16_mom16(float* master, void* m, void* v, const
   int rc = adam_args(desc, &a);
   if (rc) return rc;
   if (n <= 0) return U2_OK;
-  adamw_mom16_kernel<<<t_grid(n / 4, 256, 148LL * 16), 256, 0, ST(stream)>>>(master, BF(m), BF(v), CBF(grad), BF(param_out), n, a);
+  adamw_mom16_kernel<<<t_grid(n / 4, 256, 132LL * 16), 256, 0, ST(stream)>>>(master, BF(m), BF(v), CBF(grad), BF(param_out), n, a);
   U2_CHECK_LAUNCH("adamw");
   return U2_OK;
 }
@@ -1373,7 +1373,7 @@ extern "C" U2_API int u2_adamw_f32grad(float* master, float* m, float* v, const 
   int rc = adam_args(desc, &a);
   if (rc) return rc;
   if (n <= 0) return U2_OK;
-  adamw_kernel<true><<<t_grid(n / 4, 256, 148LL * 16), 256, 0, ST(stream)>>>(master, m, v, grad, BF(param_out_bf16), param_out_f32, n, a);
+  adamw_kernel<true><<<t_grid(n / 4, 256, 132LL * 16), 256, 0, ST(stream)>>>(master, m, v, grad, BF(param_out_bf16), param_out_f32, n, a);
   U2_CHECK_LAUNCH("adamw");
   return U2_OK;
 }
@@ -1382,7 +1382,7 @@ extern "C" U2_API int u2_sumsq_bf16(const void* x, float* out, int64_t n, void* 
   if (!x || !out) return set_error(U2_ERR_ARG, "sumsq: null pointer");
   if (n & 7) return set_error(U2_ERR_ARG, "sumsq: n must be a multiple of 8");
   if (n <= 0) return U2_OK;
-  sumsq_kernel<false><<<t_grid(n / 8, 256, 148LL * 8), 256, 0, ST(stream)>>>(x, out, n);
+  sumsq_kernel<false><<<t_grid(n / 8, 256, 132LL * 8), 256, 0, ST(stream)>>>(x, out, n);
   U2_CHECK_LAUNCH("sumsq");
   return U2_OK;
 }
@@ -1391,7 +1391,7 @@ extern "C" U2_API int u2_sumsq_f32(const float* x, float* out, int64_t n, void* 
   if (!x || !out) return set_error(U2_ERR_ARG, "sumsq: null pointer");
   if (n & 3) return set_error(U2_ERR_ARG, "sumsq: n must be a multiple of 4");
   if (n <= 0) return U2_OK;
-  sumsq_kernel<true><<<t_grid(n / 4, 256, 148LL * 8), 256, 0, ST(stream)>>>(x, out, n);
+  sumsq_kernel<true><<<t_grid(n / 4, 256, 132LL * 8), 256, 0, ST(stream)>>>(x, out, n);
   U2_CHECK_LAUNCH("sumsq");
   return U2_OK;
 }

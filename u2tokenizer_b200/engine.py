@@ -96,7 +96,7 @@ class U2Engine:
         self.pdl = os.environ.get("U2_PDL", "1") != "0"  # programmatic dependent launch between decode linears
         self.multi_op = os.environ.get("U2_MULTI_OP", "1") != "0"  # o_proj/gate-up/down/qkv chained in one launch
         self.fused_patch_embed = os.environ.get("U2_FUSED_PATCH_EMBED", "0") != "0"  # one-kernel gather + Linear (canonical patches); see DESIGN.md
-        self.use_flash = os.environ.get("U2_FLASH", "1") != "0"  # fused tcgen05 attention where it applies (dh 64)
+        self.use_flash = os.environ.get("U2_FLASH", "1") != "0"  # fused wgmma attention where it applies (dh 64)
         self.fine_deps = os.environ.get("U2_FINE_DEPS", "0") != "0"  # per-tile flags instead of grid-wide waits
         self.dl_sched = int(os.environ.get("U2_DL_SCHED", "0"))  # 1: whole 64-row tiles per CTA; 0: stream-K / 128
         self.pre_stages = int(os.environ.get("U2_PRE_STAGES", "0"))  # 0 = fill the whole ring before the dependency
@@ -255,7 +255,7 @@ class U2Engine:
         Sk, hk = k.shape[1], k.shape[2]
         Skp = _pad8(Sk)
         if dh == 64 and h == hk and rel_bias is None and not causal and self.use_flash:
-            # fused tcgen05 attention: scores never leave the SM (the ViT tower, S = 2049); V is consumed as stored
+            # fused wgmma attention: scores never leave the SM (the ViT tower, S = 2049); V is consumed as stored
             return ops.flash_attention_d64(q, k, v, out, scale)
         per_b = h * Sq * Skp * 6
         chunk = max(1, min(b, self.attn_ws // max(per_b, 1)))
@@ -295,7 +295,7 @@ class U2Engine:
         vol = frames.to(device=self.dev, dtype=F32).contiguous().view(Fr, *g.image_size)
         x = torch.empty(Fr, Sp, Hd, device=self.dev, dtype=BF16)
         if self.fused_patch_embed and ops.patch_embed_supported(g.image_size, g.patch_size, Hd):
-            # --- fused patch embedding: 5-D TMA slabs of the fp32 volume -> bf16 A operand in smem -> tcgen05 (+bias +pos)
+            # --- fused patch embedding: 5-D TMA slabs of the fp32 volume -> bf16 A operand in smem -> wgmma (+bias +pos)
             ops.patch_embed(vol, g.patch_size, self.pe_w, self.pe_b, self.pos, x)
         else:
             # --- brick gather -> GEMM (+bias +position table, rows scattered behind the cls row)
@@ -643,7 +643,7 @@ class U2Engine:
         return self.decode_impl == "tcgen05" and B <= 16 and all(k % 64 == 0 for k in dims)
 
     def decode_step_tc(self, cache: "KVCache") -> torch.Tensor:
-        """Decode step with every linear on the tcgen05 stream-K kernel and the RMSNorms folded into its
+        """Decode step with every linear on the wgmma stream-K kernel and the RMSNorms folded into its
         epilogues. Launches per step: embed, qkv(0), then per layer [fused attention, one multi-op launch
         o_proj -> gate|up -> down -> next qkv (or lm_head)], argmax  =  2 launches per layer."""
         g = self.g

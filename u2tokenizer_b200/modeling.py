@@ -9,7 +9,7 @@ Mirrors the reference classes
 with the same constructor / forward() / generate() / get_model() / initialize_vision_modules() /
 initialize_vision_tokenizer() signatures, the same state-dict keys (so reference checkpoints load with
 load_state_dict) and the same Auto* registration. The modules below only HOLD parameters; every
-forward computation is dispatched to `U2Engine` (hand-written sm_100a kernels behind the C ABI).
+forward computation is dispatched to `U2Engine` (hand-written sm_90a kernels behind the C ABI).
 Running them without CUDA / without libu2b200.so raises - there is no PyTorch fallback.
 """
 from __future__ import annotations
@@ -187,7 +187,7 @@ class U2MetaForCausalLM(ABC):
             from .engine import U2Engine
             p = next(self.parameters())
             if not p.is_cuda:
-                raise RuntimeError("the mu2 hot path runs on CUDA only: move the model to a B200 (model.cuda()); "
+                raise RuntimeError("the mu2 hot path runs on CUDA only: move the model to an H100 (model.cuda()); "
                                    "there is no CPU fallback")
             sd = {k: v for k, v in self.state_dict().items()}
             eng = U2Engine(Geometry.from_hf(self.config), sd, device=p.device)

@@ -1,6 +1,6 @@
 """Python-side operator wrappers: torch tensors in, C-ABI calls (libu2b200.so) underneath.
 
-Every function here launches hand-written sm_100a kernels on the current torch CUDA stream; none
+Every function here launches hand-written sm_90a kernels on the current torch CUDA stream; none
 of them has a PyTorch fallback. Shapes/strides are validated here, arithmetic happens in csrc/.
 """
 from __future__ import annotations
@@ -281,7 +281,7 @@ def multiscale_pool(x: torch.Tensor, gate_w: Optional[torch.Tensor], gate_bias: 
     x = x.contiguous()
     n_out = K + (K // 2 if K >= 2 else 0) + (K // 4 if K >= 4 else 0)
     out = torch.empty(B, n_out, E, device=x.device, dtype=BF16)
-    ws = torch.empty(B, 3, device=x.device, dtype=F32)
+    ws = torch.empty(int(_lib.load().u2_multiscale_pool_ws_elems(B, K)), device=x.device, dtype=F32)
     _lib.check(_lib.load().u2_multiscale_pool_bf16(x.data_ptr(), out.data_ptr(), _ptr(gate_w), gate_bias,
                                                    ws.data_ptr(), B, K, E, int(dynamic), _stream()),
                "u2_multiscale_pool_bf16")
@@ -386,8 +386,8 @@ def _dlinear_desc(x, w, out, *, ws, counters, ssq_in=None, eps=1e-6, residual=No
     _need_cuda(x, w, out, ws, counters, ssq_in, residual, gamma_next, xg, ssq_out, ssq_zero)
     d = _lib.DlinearDesc()
     d.B, d.N, d.K = x.shape[0], w.shape[0], w.shape[1]
-    if counters.numel() < (d.N + 63) // 64:
-        raise ValueError("dlinear counters too small")
+    if counters.numel() < (d.N + 63) // 64 + (ssq_out is not None):
+        raise ValueError("dlinear counters too small: ceil(N / 64) int32, + 1 with ssq_out")
     d.ws_elems = ws.numel()
     d.ldx, d.ldw, d.ldy = x.stride(0), w.stride(0), out.stride(0)
     d.ldr = residual.stride(0) if residual is not None else 0
@@ -421,7 +421,7 @@ def dlinear_new_ws(n_elems: int, device="cuda", lead=()) -> torch.Tensor:
 
 
 def dlinear(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor, **kw):
-    """Decode-step linear on tcgen05 (see u2_dlinear_desc): x [B<=16, K] bf16, w [N, K] bf16."""
+    """Decode-step linear on wgmma (see u2_dlinear_desc): x [B<=16, K] bf16, w [N, K] bf16."""
     d = _dlinear_desc(x, w, out, **kw)
     _lib.check(_lib.load().u2_dlinear_bf16(x.data_ptr(), w.data_ptr(), out.data_ptr(), C.byref(d), _stream()),
                "u2_dlinear_bf16")

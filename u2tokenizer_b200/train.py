@@ -5,7 +5,7 @@ config/ds_config.json:27-39; src/train/dpo_u2trainer.py:185-359 for stage 2) is 
 
   * `TrainEngine.forward_backward(...)`  - vision tower -> projector -> mu2-tokenizer -> splice -> decoder -> loss head,
     every activation the backward needs kept in HBM, then the backward pass: dgrad / wgrad and the attention
-    contractions on the tcgen05 GEMM (transposed operands, no copies), everything else on train_kernels.cu;
+    contractions on the wgmma GEMM (transposed operands, no copies), everything else on train_kernels.cu;
   * flat parameter / gradient buffers in a TRAINING LAYOUT (q|k|v, gate|up, wk|wv adjacent, so that one GEMM produces the
     fused gradient; every reference parameter is a contiguous slice, the nn.Parameters of the HF-style module are
     re-pointed at those slices);
@@ -467,7 +467,7 @@ class TrainEngine:
             return p_
         saved = {}
         if recompute and dh == 64 and h == hk and rel is None and not causal:
-            # fused tcgen05 attention forward (scores never leave the SM); the probabilities are recomputed in the backward
+            # fused wgmma attention forward (scores never leave the SM); the probabilities are recomputed in the backward
             lse = torch.empty(b, h, Sq, device=dev, dtype=F32)
             ops.flash_attention_d64(q, k, v, ctx, scale, lse=lse)
             saved["lse"] = lse

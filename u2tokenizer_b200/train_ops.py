@@ -183,11 +183,11 @@ def multiscale_pool_fwd(x: torch.Tensor, gate_w: Optional[torch.Tensor], dynamic
     x = x.contiguous()
     n_out = K + (K // 2 if K >= 2 else 0) + (K // 4 if K >= 4 else 0)
     out = torch.empty(B, n_out, E, device=x.device, dtype=BF16)
-    ws = torch.zeros(B, 3, device=x.device, dtype=F32)
+    ws = torch.zeros(int(_lib.load().u2_multiscale_pool_ws_elems(B, K)), device=x.device, dtype=F32)
     # gate_fc.bias shifts the three logits alike and cancels in the softmax over the scales: 0 is exact
     _lib.check(_lib.load().u2_multiscale_pool_bf16(x.data_ptr(), out.data_ptr(), _ptr(gate_w), 0.0, ws.data_ptr(), B, K, E,
                                                    int(dynamic), _stream()), "u2_multiscale_pool_bf16")
-    return out, ws
+    return out, ws[:3 * B].view(B, 3)
 
 
 def multiscale_pool_bwd(x, dy, gate_w, logits, dgate_w, dynamic: bool):
@@ -308,7 +308,7 @@ def cast(src: torch.Tensor, dst: torch.Tensor):
 
 
 # ------------------------------------------------------------------------------------------------
-# linear-layer gradients on the tcgen05 GEMM (transposed operands, no transposed copies)
+# linear-layer gradients on the wgmma GEMM (transposed operands, no transposed copies)
 # ------------------------------------------------------------------------------------------------
 def linear_dgrad(dy: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = None, *, accumulate: bool = False,
                  alpha: float = 1.0) -> torch.Tensor:
