@@ -273,6 +273,9 @@ dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
   if (warp_idx == 0) {
     // ===================== TMA producer =====================
     if (lane == 0) {
+      // every weight byte is read once per token: weight tiles are the first lines L2 gives up, so the streamed weights
+      // do not push out what is read again (activations, split-tile slots, counters, the attention's KV cache)
+      const uint64_t pol_w = l2_policy_evict_first();
       int stage = 0;
       uint32_t phase = 0;
       unsigned int target = 0;
@@ -292,7 +295,7 @@ dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
         for (int j = 0; j < npre; ++j) {
           mbar_wait(&empty_bar[st], ph ^ 1);
           mbar_arrive_expect_tx(&full_bar[st], kStageBytes);
-          tma_load_4d(smem_a + st * kABytes, &mp.tw[oi], &full_bar[st], pre.kb * kDlK, pre.tile * kM, 0, 0);
+          tma_load_4d_hint(smem_a + st * kABytes, &mp.tw[oi], &full_bar[st], pre.kb * kDlK, pre.tile * kM, 0, 0, pol_w);
           pre.next();
           if (++st == kStages) {
             st = 0;
@@ -333,7 +336,7 @@ dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
         while (it.left > 0) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
-          tma_load_4d(smem_a + stage * kABytes, &mp.tw[oi], &full_bar[stage], it.kb * kDlK, it.tile * kM, 0, 0);
+          tma_load_4d_hint(smem_a + stage * kABytes, &mp.tw[oi], &full_bar[stage], it.kb * kDlK, it.tile * kM, 0, 0, pol_w);
           if (oi > 0 && p.dep_flags) wait_tile_flag(p.dep_flags, it.kb >> p.dep_shift, step, s_ready, oi);
           tma_load_4d(smem_b + stage * kDlBBytes, &mp.tx[oi], &full_bar[stage], it.kb * kDlK, 0, 0, 0);
           it.next();

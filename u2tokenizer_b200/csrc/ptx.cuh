@@ -107,6 +107,26 @@ __device__ __forceinline__ void tma_prefetch_l2_4d(const CUtensorMap* m, int c0,
                : "memory");
 }
 
+// L2 eviction-priority policy (a 64-bit operand for the .L2::cache_hint forms below), covering the whole access.
+// evict_first: the line is the first candidate for replacement (data read once).
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+
+// tma_load_4d with an L2 cache policy
+__device__ __forceinline__ void tma_load_4d_hint(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                 int c2, int c3, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint "
+      "[%0], [%1, {%3, %4, %5, %6}], [%2], %7;"
+      :
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0),
+        "r"(c1), "r"(c2), "r"(c3), "l"(policy)
+      : "memory");
+}
+
 // 3-D tiled load (used by the patch-embed brick gather).
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
                                             int c0, int c1, int c2) {
