@@ -212,16 +212,20 @@ typedef struct u2_rope_desc {
   void* k_cache;
   void* v_cache;
   int32_t Tmax, rows_per_batch;
+  int32_t pos0_per_batch; /* != 0: pos0 = pos0_dev[row / rows_per_batch] (one position per sequence of a batch whose
+                             prompts have different lengths); 0: pos0_dev[0] (or pos0) for every row */
 } u2_rope_desc;
 U2_API int u2_rope_bf16(void* x, const u2_rope_desc* desc, void* stream);
 
 /* One query token per sequence against the KV cache (GQA). q [B, Hq*dh] (row stride ldq), caches
- * [B, Hkv, Tmax, dh]; T valid keys (or *T_dev when T_dev != NULL). Replaces the HF eager attention at q_len == 1
+ * [B, Hkv, Tmax, dh]; T valid keys (or *T_dev when T_dev != NULL; T_dev[b] for sequence b when T_per_seq != 0,
+ * which needs T_dev). Replaces the HF eager attention at q_len == 1
  * (transformers models/qwen3/modeling_qwen3.py:252-291) inside generate() (src/model/language_model/u2llama.py:123-126);
  * unfused variant used by the CUDA-core decode path. */
 U2_API int u2_decode_attention_bf16(const void* q, const void* k_cache, const void* v_cache, void* out,
                                     int32_t B, int32_t Hq, int32_t Hkv, int32_t dh, int32_t Tmax, int32_t T,
-                                    const int32_t* T_dev, int64_t ldq, int64_t ldo, float scale, void* stream);
+                                    const int32_t* T_dev, int64_t ldq, int64_t ldo, float scale, int32_t T_per_seq,
+                                    void* stream);
 
 /* Decode-step linear (weight streaming, HBM-bound): y[b, n] = sum_k norm(x)[b, k] * w[n, k] (+ residual).
  * CUDA-core variant of the HF decoder Linears (+ Qwen3RMSNorm, modeling_qwen3.py:50-67) at q_len == 1 inside generate()
@@ -333,6 +337,8 @@ typedef struct u2_fused_decode_desc {
                           keys and merges over distributed shared memory (fills the SMs when B * Hkv is small) */
   int32_t pdl;         /* != 0 (split-KV variant only): launch with programmatic stream serialisation - position read
                           and K/V prefetch overlap the tail of the preceding kernel, which must not write the cache */
+  int32_t pos_per_seq; /* != 0: sequence b appends at pos_dev[b] and attends over pos_dev[b] + 1 keys (a batch of
+                          prompts of different lengths; needs pos_dev); 0: pos_dev[0] (or pos) for every sequence */
 } u2_fused_decode_desc;
 U2_API int u2_decode_attention_fused_bf16(const void* qkv, void* k_cache, void* v_cache, void* out,
                                           const u2_fused_decode_desc* desc, void* stream);

@@ -62,6 +62,7 @@ class RopeDesc(C.Structure):
         ("pos0_dev", C.c_void_p),
         ("k_cache", C.c_void_p), ("v_cache", C.c_void_p),
         ("Tmax", C.c_int32), ("rows_per_batch", C.c_int32),
+        ("pos0_per_batch", C.c_int32),
     ]
 
 
@@ -113,6 +114,7 @@ class FusedDecodeDesc(C.Structure):
         ("inv_freq", C.c_void_p),
         ("scale", C.c_float),
         ("kv_splits", C.c_int32), ("pdl", C.c_int32),
+        ("pos_per_seq", C.c_int32),
     ]
 
 
@@ -211,7 +213,7 @@ SIGNATURES = {
     "u2_embed_splice_bf16": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _L, _P]),
     "u2_temporal_attention_bf16": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _L, _L, _F, _P, _I, _P]),
     "u2_rope_bf16": (C.c_int, [_P, C.POINTER(RopeDesc), _P]),
-    "u2_decode_attention_bf16": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _L, _L, _F, _P]),
+    "u2_decode_attention_bf16": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _L, _L, _F, _I, _P]),
     "u2_gemv_bf16": (C.c_int, [_P, _P, _P, C.POINTER(GemvDesc), _P]),
     "u2_argmax_f32": (C.c_int, [_P, _P, _P, _I, _I, _L, _P]),
     "u2_dlinear_bf16": (C.c_int, [_P, _P, _P, C.POINTER(DlinearDesc), _P]),

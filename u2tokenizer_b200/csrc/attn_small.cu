@@ -121,6 +121,7 @@ struct RopeArgs {
   __nv_bfloat16* k_cache;    // [B, n_k_heads, Tmax, dh] or null
   __nv_bfloat16* v_cache;
   int Tmax, rows_per_batch;  // batch index = row / rows_per_batch, cache position = position(row)
+  int pos0_per_batch;        // pos0 = pos0_dev[batch index] instead of pos0_dev[0]
 };
 
 __global__ void __launch_bounds__(256)
@@ -132,11 +133,12 @@ rope_kernel(const RopeArgs a) {
   const long long row = item / heads;
   const int head = (int)(item - row * heads);
   __nv_bfloat16* p = a.x + row * a.ld + (long long)head * a.dh;
-  const int pos = (a.pos0_dev ? *a.pos0_dev : a.pos0) + (int)((row / a.pos_div) % a.pos_mod);
+  const int b = (int)(row / a.rows_per_batch);
+  const int pos0 = a.pos0_dev ? a.pos0_dev[a.pos0_per_batch ? b : 0] : a.pos0;
+  const int pos = pos0 + (int)((row / a.pos_div) % a.pos_mod);
   const int half = a.dh >> 1;
   const bool is_q = head < a.n_q_heads;
   const bool is_k = !is_q && head < a.n_q_heads + a.n_k_heads;
-  const int b = (int)(row / a.rows_per_batch);
   if (!is_q && !is_k) {
     if (a.v_cache) {
       const int hv = head - a.n_q_heads - a.n_k_heads;
@@ -205,10 +207,10 @@ __global__ void __launch_bounds__(256)
 decode_attention_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
                         const __nv_bfloat16* __restrict__ vc, __nv_bfloat16* __restrict__ out, int Hq, int Hkv,
                         int Tmax, int T_host, const int* __restrict__ T_dev, long long ldq, long long ldo,
-                        float scale) {
+                        float scale, int T_per_seq) {
   constexpr int dh = kEpl * 32;
-  const int T = T_dev ? min(*T_dev, Tmax) : T_host;
   const int h = blockIdx.x, b = blockIdx.y;
+  const int T = T_dev ? min(T_dev[T_per_seq ? b : 0], Tmax) : T_host;
   const int hk = h / (Hq / Hkv);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const __nv_bfloat16* qp = q + (long long)b * ldq + (long long)h * dh + lane * kEpl;
@@ -300,6 +302,7 @@ extern "C" U2_API int u2_rope_bf16(void* x, const u2_rope_desc* d, void* stream)
     return set_error(U2_ERR_ARG, "rope: cache append needs Tmax and rows_per_batch");
   if (d->k_cache && !d->pos0_dev && d->pos0 + d->pos_mod > d->Tmax)
     return set_error(U2_ERR_ARG, "rope: cache overflow (pos0 %d + %d > Tmax %d)", d->pos0, d->pos_mod, d->Tmax);
+  if (d->pos0_per_batch && !d->pos0_dev) return set_error(U2_ERR_ARG, "rope: pos0_per_batch needs pos0_dev");
   RopeArgs a;
   a.x = BF(x);
   a.rows = d->rows; a.ld = d->ld; a.dh = d->dh;
@@ -310,6 +313,7 @@ extern "C" U2_API int u2_rope_bf16(void* x, const u2_rope_desc* d, void* stream)
   a.pos0 = d->pos0; a.pos_div = d->pos_div > 0 ? d->pos_div : 1; a.pos_mod = d->pos_mod > 0 ? d->pos_mod : 1;
   a.k_cache = BF(d->k_cache); a.v_cache = BF(d->v_cache);
   a.Tmax = d->Tmax; a.rows_per_batch = d->rows_per_batch > 0 ? d->rows_per_batch : 1;
+  a.pos0_per_batch = d->pos0_per_batch != 0;
   const long long items = d->rows * (long long)(a.n_q_heads + a.n_k_heads + a.n_v_heads);
   rope_kernel<<<(unsigned)((items + 7) / 8), 256, 0, ST(stream)>>>(a);
   U2_CHECK_LAUNCH("rope");
@@ -319,12 +323,13 @@ extern "C" U2_API int u2_rope_bf16(void* x, const u2_rope_desc* d, void* stream)
 extern "C" U2_API int u2_decode_attention_bf16(const void* q, const void* k_cache, const void* v_cache, void* out,
                                                int32_t B, int32_t Hq, int32_t Hkv, int32_t dh, int32_t Tmax,
                                                int32_t T, const int32_t* T_dev, int64_t ldq, int64_t ldo,
-                                               float scale, void* stream) {
+                                               float scale, int32_t T_per_seq, void* stream) {
   if (!q || !k_cache || !v_cache || !out) return set_error(U2_ERR_ARG, "decode_attention: null pointer");
   if (Hkv <= 0 || Hq % Hkv) return set_error(U2_ERR_ARG, "decode_attention: Hq must be a multiple of Hkv");
   if (!T_dev && (T <= 0 || T > Tmax)) return set_error(U2_ERR_ARG, "decode_attention: need 0 < T <= Tmax");
+  if (T_per_seq && !T_dev) return set_error(U2_ERR_ARG, "decode_attention: T_per_seq needs T_dev");
   dim3 grid((unsigned)Hq, (unsigned)B);
-#define U2_DA(EPL) decode_attention_kernel<EPL><<<grid, 256, 0, ST(stream)>>>(CBF(q), CBF(k_cache), CBF(v_cache), BF(out), Hq, Hkv, Tmax, T, T_dev, ldq, ldo, scale)
+#define U2_DA(EPL) decode_attention_kernel<EPL><<<grid, 256, 0, ST(stream)>>>(CBF(q), CBF(k_cache), CBF(v_cache), BF(out), Hq, Hkv, Tmax, T, T_dev, ldq, ldo, scale, T_per_seq != 0)
   switch (dh) {
     case 32: U2_DA(1); break;
     case 64: U2_DA(2); break;
@@ -362,6 +367,7 @@ struct FusedDecodeArgs {
   long long ldo;
   int Hq, Hkv, Tmax;
   const int* pos_dev;        // position of the new token (device); T = pos + 1
+  int pos_per_seq;           // pos = pos_dev[sequence] instead of pos_dev[0]
   int pos_host;
   const float* q_norm_w;     // [dh] or null
   const float* k_norm_w;
@@ -418,7 +424,7 @@ fused_decode_attention_kernel(const FusedDecodeArgs a) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   asm volatile("griddepcontrol.wait;" ::: "memory");  // PDL: the QKV projection must have landed
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // o_proj may start prefetching its weights
-  const int pos = a.pos_dev ? *a.pos_dev : a.pos_host;
+  const int pos = a.pos_dev ? a.pos_dev[a.pos_per_seq ? b : 0] : a.pos_host;
   const int T = min(pos + 1, a.Tmax);
   __shared__ __align__(16) float s_q[kG][kDh];
   __shared__ float s_m[kFaWarps][kG], s_l[kFaWarps][kG];
@@ -569,8 +575,9 @@ fused_decode_attention_split_kernel(const FusedDecodeArgs a) {
   // PDL: the kernel behind us (the next chained decode-linear launch) may start its prologue and weight prefetch
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   // the position is advanced at the end of the previous decode step, several fully serialised launches ago: safe to
-  // read before the dependency wait, like the cache rows below the new position
-  const int pos = a.pos_dev ? *a.pos_dev : a.pos_host;
+  // read before the dependency wait, like the cache rows below the new position. b is uniform over the cluster (it
+  // spans z only), so every CTA of a cluster sees the same T
+  const int pos = a.pos_dev ? a.pos_dev[a.pos_per_seq ? b : 0] : a.pos_host;
   const int T = min(pos + 1, a.Tmax);
   __shared__ __align__(16) float s_q[kG][kDh];
   __shared__ __align__(16) __nv_bfloat16 s_knew[kDh];
@@ -811,12 +818,13 @@ extern "C" U2_API int u2_decode_attention_fused_bf16(const void* qkv, void* k_ca
   if (d->Hkv <= 0 || d->Hq % d->Hkv || d->Hq / d->Hkv > kFaMaxG)
     return set_error(U2_ERR_UNSUPPORTED, "decode_attention_fused: Hq/Hkv must be an integer <= %d", kFaMaxG);
   if (!d->pos_dev && (d->pos < 0 || d->pos >= d->Tmax)) return set_error(U2_ERR_ARG, "decode_attention_fused: position outside the cache");
+  if (d->pos_per_seq && !d->pos_dev) return set_error(U2_ERR_ARG, "decode_attention_fused: pos_per_seq needs pos_dev");
   FusedDecodeArgs a;
   a.qkv = CBF(qkv); a.ldq = d->ldq;
   a.kc = BF(k_cache); a.vc = BF(v_cache);
   a.out = BF(out); a.ldo = d->ldo;
   a.Hq = d->Hq; a.Hkv = d->Hkv; a.Tmax = d->Tmax;
-  a.pos_dev = d->pos_dev; a.pos_host = d->pos;
+  a.pos_dev = d->pos_dev; a.pos_per_seq = d->pos_per_seq != 0; a.pos_host = d->pos;
   a.q_norm_w = d->q_norm_w; a.k_norm_w = d->k_norm_w; a.eps = d->eps;
   a.inv_freq = d->inv_freq; a.scale = d->scale;
   const int splits = d->kv_splits > 1 ? d->kv_splits : 1;

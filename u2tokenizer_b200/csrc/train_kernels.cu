@@ -1237,6 +1237,7 @@ extern "C" U2_API int u2_rope_bwd_bf16(void* dx, const void* x_raw, const u2_rop
   if (!dx || !d || !d->inv_freq) return set_error(U2_ERR_ARG, "rope_bwd: null pointer");
   if (d->dh <= 0 || (d->dh & 1) || (d->ld & 1)) return set_error(U2_ERR_ARG, "rope_bwd: head_dim and ld must be even");
   if ((d->q_norm_w || d->k_norm_w) && !x_raw) return set_error(U2_ERR_ARG, "rope_bwd: the per-head norm backward needs the raw projections");
+  if (d->pos0_per_batch) return set_error(U2_ERR_UNSUPPORTED, "rope_bwd: per-batch positions are a decode-only feature");
   if (d->rows <= 0) return U2_OK;
   RopeBwdArgs a;
   a.dx = BF(dx); a.x_raw = CBF(x_raw);

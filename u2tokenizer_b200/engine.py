@@ -663,7 +663,7 @@ class U2Engine:
             ops.decode_attention_fused(qkv, cache.k[li], cache.v[li], ctx, B=B, Hq=hq, Hkv=hkv, dh=dh, Tmax=cache.max_len,
                                        inv_freq=self.inv_freq, scale=1.0 / math.sqrt(dh), pos_dev=cache.length_dev,
                                        q_norm_w=w["qn"], k_norm_w=w["kn"], eps=eps, kv_splits=self._kv_splits(B),
-                                       pdl=self.pdl and self.attn_pdl)
+                                       pdl=self.pdl and self.attn_pdl, pos_per_seq=True)
             last = li + 1 == nl
             g_next = self.final_norm if last else self.layers[li + 1]["ln1"]
             fl = flags[li] if (self.multi_op and self.fine_deps) else [None] * 4
@@ -714,8 +714,8 @@ class U2Engine:
         return self._samp_dev
 
     def decode_step(self, cache: "KVCache") -> torch.Tensor:
-        """Consumes buffers['ids'] [B,1] (the last token of every sequence), appends to the cache at
-        position cache.length (read on the device), leaves fp32 logits in buffers['logits'] and the greedy
+        """Consumes buffers['ids'] [B,1] (the last token of every sequence), appends sequence b to the cache at
+        position cache.length_dev[b] (read on the device), leaves fp32 logits in buffers['logits'] and the greedy
         next ids back in buffers['ids']. Launch sequence is CUDA-graph capturable."""
         g = self.g
         B = cache.batch
@@ -730,9 +730,10 @@ class U2Engine:
             ops.gemv(x, w["wqkv"], qkv, norm_gamma=w["ln1"], norm_eps=g.rms_norm_eps)
             ops.rope(qkv, rows=B, ld=nqkv, dh=dh, n_q=hq, n_k=hkv, n_v=hkv, inv_freq=self.inv_freq, q_norm_w=w["qn"],
                      k_norm_w=w["kn"], eps=g.rms_norm_eps, pos0=0, pos_div=1, pos_mod=1, pos0_dev=cache.length_dev,
-                     k_cache=cache.k[li], v_cache=cache.v[li], Tmax=cache.max_len, rows_per_batch=1)
+                     k_cache=cache.k[li], v_cache=cache.v[li], Tmax=cache.max_len, rows_per_batch=1, pos0_per_batch=True)
             ops.decode_attention(qkv, cache.k[li], cache.v[li], ctx, B=B, Hq=hq, Hkv=hkv, dh=dh, Tmax=cache.max_len,
-                                 T_dev=cache.length_plus1_dev, ldq=nqkv, ldo=hq * dh, scale=1.0 / math.sqrt(dh))
+                                 T_dev=cache.length_plus1_dev, ldq=nqkv, ldo=hq * dh, scale=1.0 / math.sqrt(dh),
+                                 T_per_seq=True)
             ops.gemv(ctx, w["wo"], x, residual=x)
             ops.gemv(x, w["wgu"], act, norm_gamma=w["ln2"], norm_eps=g.rms_norm_eps, silu_pair=True)
             ops.gemv(act, w["wdown"], x, residual=x)
@@ -748,21 +749,27 @@ class U2Engine:
     @torch.no_grad()
     def generate(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id=None, do_sample: bool = False,
                  temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, seed: int = 0, use_graph: bool = True,
-                 num_return_sequences: int = 1):
+                 num_return_sequences: int = 1, lengths=None):
         """Greedy (do_sample=False) or sampled decoding; same loop, only the token-picking head differs.
         num_return_sequences > 1 (HF semantics: row b * n + s is sample s of prompt b) shares ONE vision + prefill pass:
         the prompt's KV rows are replicated into the decode cache (the reference's DPO-data workflow draws 8 samples per
-        study by re-running the whole model per sample, green_refactored/pred_then_green.py:77-83)."""
+        study by re-running the whole model per sample, green_refactored/pred_then_green.py:77-83).
+        lengths [B] (optional): prompt b is embeds[b, :lengths[b]] (right padding after it); it decodes from position
+        lengths[b] on, as if it ran alone. None = every prompt fills the whole width."""
         self._sampling = dict(temperature=float(temperature), top_k=int(top_k or 0), top_p=float(top_p),
                               seed=int(seed)) if do_sample else None
         try:
+            lens = self._row_lengths(lengths, embeds.shape[0], embeds.shape[1])
             if num_return_sequences > 1:
-                return self._generate_multi(embeds, max_new_tokens, eos_token_id, use_graph, int(num_return_sequences))
+                return self._generate_multi(embeds, max_new_tokens, eos_token_id, use_graph, int(num_return_sequences),
+                                            lengths=lens)
             cap = 16 if self._use_tc_decode(16) else 8  # sequences one decode step can carry (dlinear N / gemv batch)
             if embeds.shape[0] <= cap:
-                return self.generate_greedy(embeds, max_new_tokens, eos_token_id=eos_token_id, use_graph=use_graph)
+                return self.generate_greedy(embeds, max_new_tokens, eos_token_id=eos_token_id, use_graph=use_graph,
+                                            lengths=lens)
             outs = [self.generate_greedy(embeds[b0:b0 + cap].contiguous(), max_new_tokens, eos_token_id=eos_token_id,
-                                         use_graph=use_graph) for b0 in range(0, embeds.shape[0], cap)]
+                                         use_graph=use_graph, lengths=lens[b0:b0 + cap])
+                    for b0 in range(0, embeds.shape[0], cap)]
             width = max(o.shape[1] for o in outs)
             if any(o.shape[1] != width for o in outs):  # chunks that hit EOS early: pad with EOS (masked by the caller)
                 fill = eos_token_id[0] if isinstance(eos_token_id, (list, tuple)) else eos_token_id
@@ -782,42 +789,67 @@ class U2Engine:
             self._gen_state = st
         return st
 
+    @staticmethod
+    def _row_lengths(lengths, B: int, L: int) -> torch.Tensor:
+        """Per-row prompt lengths as a CPU int64 tensor [B] (None: every row is L long)."""
+        if lengths is None:
+            return torch.full((B,), L, dtype=torch.int64)
+        lens = torch.as_tensor(lengths).to(device="cpu", dtype=torch.int64).reshape(-1)
+        if lens.numel() != B:
+            raise ValueError(f"lengths has {lens.numel()} entries for a batch of {B} prompts")
+        if bool((lens < 1).any()) or bool((lens > L).any()):
+            raise ValueError(f"prompt lengths {lens.tolist()} outside 1..{L} (the padded width)")
+        return lens
+
+    def _last_hidden(self, hidden: torch.Tensor, lens: torch.Tensor) -> torch.Tensor:
+        """hidden[b, lens[b] - 1] for every row: the state the first new token of prompt b is picked from."""
+        B = hidden.shape[0]
+        return hidden[torch.arange(B, device=hidden.device), (lens - 1).to(hidden.device)]
+
     def generate_greedy(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id=None,
                         use_graph: bool = True, return_margins: bool = False, force_ids: Optional[torch.Tensor] = None,
-                        logits_out: Optional[list] = None):
+                        logits_out: Optional[list] = None, lengths=None):
         """Prefill on `embeds` [B, L, E], then max_new_tokens decode steps (greedy unless a sampling configuration
         was installed by generate()). Returns new ids [B, n] (and the per-step top-1/top-2 logit margins when
         asked, for margin-aware parity checks).
         force_ids [B, n] (parity tests): teacher forcing - the returned ids are still this engine's own picks, but the
         token fed to the next step is force_ids[:, step], so one near-tie cannot derail the rest of the comparison.
-        logits_out: a list that receives a copy of every step's fp32 logits [B, V]."""
+        logits_out: a list that receives a copy of every step's fp32 logits [B, V].
+        lengths [B] (optional): prompt b is embeds[b, :lengths[b]]. The prefill runs over the padded width; causal
+        attention keeps the real positions exact, and the cache rows from lengths[b] on are overwritten by the decode
+        steps before any step reads them."""
         B, L, _ = embeds.shape
+        lens = self._row_lengths(lengths, B, L)
         st = self._gen_state_for(B, L + max_new_tokens)
         cache = st["cache"]
         cache.set_length(0)
         hidden = self.prefill(embeds, cache)
-        logits0 = self.lm_logits(hidden[:, -1].contiguous())
+        cache.set_length(lens)
+        logits0 = self.lm_logits(self._last_hidden(hidden, lens))
         return self._decode_loop(st, logits0, max_new_tokens, eos_token_id, use_graph, return_margins,
                                  force_ids=force_ids, logits_out=logits_out)
 
-    def _generate_multi(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id, use_graph: bool, n: int):
+    def _generate_multi(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id, use_graph: bool, n: int,
+                        lengths=None):
         B, L, _ = embeds.shape
+        lens = self._row_lengths(lengths, B, L)
         pc = self.new_cache(B, L)
         hidden = self.prefill(embeds, pc)
-        logits0 = self.lm_logits(hidden[:, -1].contiguous())
+        logits0 = self.lm_logits(self._last_hidden(hidden, lens))
         rows = B * n
         chunk = 16 if self._use_tc_decode(16) else 8  # sequences one decode step can carry (dlinear N / gemv batch)
         base = dict(self._sampling) if self._sampling else None
         outs = []
         for ci, c0 in enumerate(range(0, rows, chunk)):
-            src = torch.arange(c0, min(rows, c0 + chunk), device=self.dev) // n  # prompt of every row of this chunk
+            src_cpu = torch.arange(c0, min(rows, c0 + chunk)) // n  # prompt of every row of this chunk
+            src = src_cpu.to(self.dev)
             if base is not None:  # distinct random streams per chunk (the sampler keys its stream by (seed, step, row))
                 self._sampling = dict(base, seed=(base["seed"] + 0x9E3779B97F4A7C15 * ci) & ((1 << 64) - 1))
             st = self._gen_state_for(int(src.numel()), L + max_new_tokens)
             cache = st["cache"]
             cache.k[:, :, :, :L].copy_(pc.k.index_select(1, src))
             cache.v[:, :, :, :L].copy_(pc.v.index_select(1, src))
-            cache.set_length(L)
+            cache.set_length(lens.index_select(0, src_cpu))  # every sample continues from its prompt's length
             outs.append(self._decode_loop(st, logits0.index_select(0, src), max_new_tokens, eos_token_id, use_graph, False))
         width = max(o.shape[1] for o in outs)
         if any(o.shape[1] != width for o in outs):  # chunks that hit EOS early: pad with EOS (masked by the caller)
@@ -891,8 +923,9 @@ class U2Engine:
 
 
 class KVCache:
-    """Static KV cache [layers][B, Hkv, Tmax, dh] bf16 + the current length on the device (so the decode
-    step's launch parameters never change and the step can live in a CUDA graph)."""
+    """Static KV cache [layers][B, Hkv, Tmax, dh] bf16 + the current length of every sequence on the device
+    (int32 [B], so the decode step's launch parameters never change and the step can live in a CUDA graph; prompts of
+    different lengths decode side by side, each at its own position). `length` is the longest row's length."""
 
     def __init__(self, g: Geometry, batch: int, max_len: int, device):
         self.batch, self.max_len = batch, max_len
@@ -900,13 +933,26 @@ class KVCache:
         self.k = torch.zeros(shape, device=device, dtype=BF16)
         self.v = torch.zeros(shape, device=device, dtype=BF16)
         self.length = 0
-        self.length_dev = torch.zeros(1, device=device, dtype=torch.int32)
-        self.length_plus1_dev = torch.ones(1, device=device, dtype=torch.int32)
+        self.length_dev = torch.zeros(batch, device=device, dtype=torch.int32)
+        self.length_plus1_dev = torch.ones(batch, device=device, dtype=torch.int32)
 
-    def set_length(self, n: int):
-        self.length = n
-        self.length_dev.fill_(n)
-        self.length_plus1_dev.fill_(n + 1)
+    def set_length(self, n):
+        """n: one length for every sequence, or the per-sequence lengths [B]."""
+        lens = torch.as_tensor(n)
+        if lens.dim() == 0:
+            n = int(lens)
+            self.length = n
+            self.length_dev.fill_(n)
+            self.length_plus1_dev.fill_(n + 1)
+            return
+        lens = lens.to(device="cpu", dtype=torch.int32).reshape(-1)
+        if lens.numel() != self.batch:
+            raise ValueError(f"{lens.numel()} lengths for a cache of {self.batch} sequences")
+        if bool((lens < 0).any()) or bool((lens > self.max_len).any()):
+            raise ValueError(f"lengths {lens.tolist()} outside 0..{self.max_len}")
+        self.length = int(lens.max())
+        self.length_dev.copy_(lens)
+        self.length_plus1_dev.copy_(lens + 1)
 
     def advance_device(self):
         self.length_dev.add_(1)

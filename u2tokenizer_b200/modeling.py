@@ -294,6 +294,37 @@ class U2MetaForCausalLM(ABC):
             raise NotImplementedError("attention_mask must be all ones or right-padded (left-padded / sparse masks are "
                                       "not supported by the fused CUDA path)")
 
+    @staticmethod
+    def _generate_prompt_rows(input_ids, attention_mask, min_len: int = 1):
+        """generate()'s padded batch -> (input_ids with every row's real tokens moved to the front, per-row lengths
+        [B] int64 on the CPU). The lengths are None when the mask is absent or all ones (every prompt fills the width).
+        A row is right-padded (its ones start at column 0) or left-padded (they end at the last column, as trl's
+        collator pads prompts); left padding is rolled to the right BEFORE the visual tokens are spliced at positions
+        1..n_vis, so each row sees the positions it would see alone. min_len: <bos> + the visual tokens."""
+        if attention_mask is None:
+            return input_ids, None
+        m = attention_mask.detach().to("cpu", torch.bool)
+        if m.dim() != 2 or tuple(m.shape) != tuple(input_ids.shape):
+            raise ValueError(f"attention_mask {tuple(m.shape)} does not match input_ids {tuple(input_ids.shape)}")
+        if bool(m.all()):
+            return input_ids, None
+        B, L = m.shape
+        lens = m.sum(dim=1)
+        col = torch.arange(L)
+        right = (m == (col[None, :] < lens[:, None])).all(dim=1)
+        left = (m == (col[None, :] >= (L - lens)[:, None])).all(dim=1)
+        if not bool((right | left).all()):
+            raise NotImplementedError("attention_mask must be all ones, right-padded or left-padded in generate() "
+                                      "(masks with holes are not supported by the fused CUDA path)")
+        short = (lens < min_len).nonzero().flatten().tolist()
+        if short:
+            raise ValueError(f"prompt rows {short} have {lens[short].tolist()} tokens: each needs at least {min_len} "
+                             "(<bos> + the visual tokens)")
+        shift = torch.where(right, torch.zeros_like(lens), L - lens)  # left-padded rows: real tokens start at L - len
+        idx = (col[None, :] + shift[:, None]) % L
+        ids = input_ids.gather(1, idx.to(input_ids.device))
+        return ids, lens
+
     # ---- forward / generate shared by the Llama and Qwen3 wrappers (reference u2llama.py:41-138) ----
     def _u2_forward(self, images=None, input_ids=None, labels=None, attention_mask=None, question_ids=None,
                     position_ids=None, past_key_values=None, inputs_embeds=None, use_cache=None,
@@ -380,6 +411,13 @@ class U2MetaForCausalLM(ABC):
         if "inputs_embeds" in kwargs:
             raise NotImplementedError("`inputs_embeds` is not supported")
         eng = self.engine()
+        # prompts of different lengths: real tokens first, one length per row (the decode runs each row at its own
+        # positions); the reference drops the mask here (u2llama.py:97-99) and would decode after the pads
+        if inputs is None:
+            raise ValueError("generate() needs input_ids")
+        splices = images is not None and self.get_vision_tower() is not None and inputs.shape[1] != 1
+        n_vis = (eng.g.num_3d_query_token if eng.g.enable_u2tokenizer else eng.g.tokens_per_frame) if splices else 0
+        inputs, lengths = self._generate_prompt_rows(inputs, attention_mask, min_len=1 + n_vis)
         if images is not None:
             (inputs, position_ids, attention_mask, _, inputs_embeds, _
              ) = self.prepare_inputs_for_multimodal(inputs, position_ids, attention_mask, None, None, images, question_ids)
@@ -442,7 +480,7 @@ class U2MetaForCausalLM(ABC):
             raise ValueError("num_return_sequences > 1 needs do_sample=True (greedy decoding is deterministic; HF raises too)")
         ids = eng.generate(inputs_embeds.to(torch.bfloat16), max_new_tokens=max_new, eos_token_id=eos,
                            do_sample=bool(do_sample), temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
-                           num_return_sequences=n_ret)
+                           num_return_sequences=n_ret, lengths=lengths)
         if eos is not None:
             eos_t = torch.as_tensor(eos if isinstance(eos, (list, tuple)) else [eos], device=ids.device)
             hit = torch.isin(ids, eos_t)

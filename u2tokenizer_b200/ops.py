@@ -321,7 +321,8 @@ def temporal_attention(qkv: torch.Tensor, out: torch.Tensor, *, B: int, C_: int,
 def rope(x: torch.Tensor, *, rows: int, ld: int, dh: int, n_q: int, n_k: int, n_v: int = 0,
          inv_freq: torch.Tensor, q_norm_w=None, k_norm_w=None, eps: float = 1e-6,
          pos0: int = 0, pos_div: int = 1, pos_mod: int = 1, pos0_dev=None,
-         k_cache=None, v_cache=None, Tmax: int = 0, rows_per_batch: int = 1):
+         k_cache=None, v_cache=None, Tmax: int = 0, rows_per_batch: int = 1, pos0_per_batch: bool = False):
+    """pos0_per_batch: pos0 = pos0_dev[row // rows_per_batch] (int32 [batch], one position per sequence)."""
     _need_cuda(x, inv_freq, q_norm_w, k_norm_w, k_cache, v_cache, pos0_dev)
     d = _lib.RopeDesc()
     d.rows, d.ld, d.dh = rows, ld, dh
@@ -332,17 +333,19 @@ def rope(x: torch.Tensor, *, rows: int, ld: int, dh: int, n_q: int, n_k: int, n_
     d.pos0_dev = _ptr(pos0_dev)
     d.k_cache, d.v_cache = _ptr(k_cache), _ptr(v_cache)
     d.Tmax, d.rows_per_batch = Tmax, rows_per_batch
+    d.pos0_per_batch = 1 if pos0_per_batch else 0
     _lib.check(_lib.load().u2_rope_bf16(x.data_ptr(), C.byref(d), _stream()), "u2_rope_bf16")
     return x
 
 
 def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, out: torch.Tensor, *,
                      B: int, Hq: int, Hkv: int, dh: int, Tmax: int, T: int = 0, T_dev=None, ldq: int, ldo: int,
-                     scale: float):
+                     scale: float, T_per_seq: bool = False):
+    """T_per_seq: sequence b attends over T_dev[b] keys (int32 [B])."""
     _need_cuda(q, k_cache, v_cache, out, T_dev)
     _lib.check(_lib.load().u2_decode_attention_bf16(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                                     out.data_ptr(), B, Hq, Hkv, dh, Tmax, T, _ptr(T_dev), ldq, ldo,
-                                                    scale, _stream()), "u2_decode_attention_bf16")
+                                                    scale, 1 if T_per_seq else 0, _stream()), "u2_decode_attention_bf16")
     return out
 
 
@@ -463,9 +466,10 @@ def decode_embed(ids: torch.Tensor, table: torch.Tensor, gamma: torch.Tensor, x:
 def decode_attention_fused(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, out: torch.Tensor, *,
                            B: int, Hq: int, Hkv: int, dh: int, Tmax: int, inv_freq: torch.Tensor, scale: float,
                            pos: int = 0, pos_dev=None, q_norm_w=None, k_norm_w=None, eps: float = 1e-6, kv_splits: int = 1,
-                           pdl: bool = False):
+                           pdl: bool = False, pos_per_seq: bool = False):
     """q/k norm + RoPE + KV-cache append + GQA attention for one new token per sequence (one launch).
-    kv_splits in {2, 4, 8}: a cluster of that many CTAs per (sequence, KV head) splits the cached keys."""
+    kv_splits in {2, 4, 8}: a cluster of that many CTAs per (sequence, KV head) splits the cached keys.
+    pos_per_seq: sequence b's new token sits at position pos_dev[b] (int32 [B]) instead of pos_dev[0]."""
     _need_cuda(qkv, k_cache, v_cache, out, inv_freq, pos_dev, q_norm_w, k_norm_w)
     d = _lib.FusedDecodeDesc()
     d.B, d.Hq, d.Hkv, d.dh, d.Tmax, d.pos = B, Hq, Hkv, dh, Tmax, pos
@@ -476,6 +480,7 @@ def decode_attention_fused(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: to
     d.scale = scale
     d.kv_splits = int(kv_splits)
     d.pdl = 1 if pdl else 0
+    d.pos_per_seq = 1 if pos_per_seq else 0
     _lib.check(_lib.load().u2_decode_attention_fused_bf16(qkv.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                                           out.data_ptr(), C.byref(d), _stream()),
                "u2_decode_attention_fused_bf16")
