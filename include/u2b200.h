@@ -390,6 +390,42 @@ typedef struct u2_sample_params {
 U2_API int u2_sample_dev_f32(const float* logits, int64_t* out, int32_t B, int32_t V, int64_t ld,
                              const u2_sample_params* params_dev, const int32_t* step_dev, int32_t step, void* stream);
 
+/* Logits processors of HF generate(repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_new_tokens /
+ * min_length), in place on logits [B, V] (row stride ld) before u2_argmax_f32 / u2_sample_dev_f32. Replaces, in this
+ * order, RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor, NoBadWordsLogitsProcessor and
+ * MinLengthLogitsProcessor / MinNewTokensLengthLogitsProcessor (transformers generation/logits_process.py, built by
+ * GenerationMixin._get_logits_processor; reference call src/model/language_model/u2llama.py:123-126).
+ * History: t = *step_dev (or step when step_dev is NULL) generated tokens, t <= hist_cap. When t > 0 the token fed to
+ * this step, ids[b], is first stored at hist[b * ld_hist + t - 1]; the processors then read hist[b, 0..t-1]. A decode
+ * step that bumps *step_dev before this launch can therefore be captured in a CUDA graph.
+ *   penalty != 1: every distinct history token v gets x < 0 ? x * penalty : x * inv_penalty, from its unprocessed x
+ *                 (inv_penalty = fp32(1 / fp32(penalty)), which is how torch evaluates `scores / penalty` on CUDA);
+ *   ngram = n > 0: hist[i + n - 1] -> -inf for every i with hist[i .. i+n-2] == hist[t-n+1 .. t-1];
+ *   bad words:    word w is bad_tok[bad_off[w] .. bad_off[w+1]); a one-token word is always -inf, a longer word bans its
+ *                 last token when its length is <= t and its prefix equals the end of the history; -0.0 becomes +0.0
+ *                 in every row (HF adds a 0 / -inf bias row);
+ *   min_new:      eos[0 .. n_eos) -> -inf while t < min_new.
+ * The parameters live in DEVICE memory (like u2_sample_params): a captured step picks up a new request's values from
+ * one host-to-device copy. The caller validates them: penalty > 0, ngram >= 0, every token id in [0, V), n_bad words
+ * of at least one token within the capacities below. Dynamic shared memory: one bit per vocabulary entry. */
+#define U2_LP_MAX_EOS 8
+#define U2_LP_MAX_BAD_WORDS 256
+#define U2_LP_MAX_BAD_TOKENS 2048
+typedef struct u2_logits_proc_params {
+  float penalty;     /* 1.0: off */
+  float inv_penalty;
+  int32_t ngram;     /* 0: off */
+  int32_t min_new;   /* 0: off */
+  int32_t n_eos;
+  int32_t n_bad;     /* 0: off */
+  int32_t eos[U2_LP_MAX_EOS];
+  int32_t bad_off[U2_LP_MAX_BAD_WORDS + 1];
+  int32_t bad_tok[U2_LP_MAX_BAD_TOKENS];
+} u2_logits_proc_params;
+U2_API int u2_logits_process_f32(float* logits, int32_t B, int32_t V, int64_t ld, const int64_t* ids, int32_t* hist,
+                                 int64_t ld_hist, int32_t hist_cap, const u2_logits_proc_params* params_dev,
+                                 const int32_t* step_dev, int32_t step, void* stream);
+
 /* Fused lm_head + selective log-softmax (the DPO / SFT log-probability head) -----------------------------------
  * logp[r] = log_softmax(hidden[r] . W^T)[labels[r]]  (0 where labels[r] < 0) without materialising the [R, V] logits:
  * the GEMM's epilogue reduces every 128-column half tile to (max, sum exp, sum) per row, a second small kernel merges

@@ -190,6 +190,20 @@ class AdamWDesc(C.Structure):
     ]
 
 
+LP_MAX_EOS, LP_MAX_BAD_WORDS, LP_MAX_BAD_TOKENS = 8, 256, 2048  # U2_LP_MAX_* of include/u2b200.h
+
+
+class LogitsProcParams(C.Structure):
+    """Mirror of ``u2_logits_proc_params`` (copied to device memory as raw bytes)."""
+    _fields_ = [
+        ("penalty", C.c_float), ("inv_penalty", C.c_float), ("ngram", C.c_int32), ("min_new", C.c_int32),
+        ("n_eos", C.c_int32), ("n_bad", C.c_int32),
+        ("eos", C.c_int32 * LP_MAX_EOS),
+        ("bad_off", C.c_int32 * (LP_MAX_BAD_WORDS + 1)),
+        ("bad_tok", C.c_int32 * LP_MAX_BAD_TOKENS),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/u2b200.h / u2b200_train.h declares must be listed here
 # (tests/test_abi.py cross-checks this table against the header and the built library).
 _P, _I, _L, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
@@ -222,6 +236,7 @@ SIGNATURES = {
     "u2_flash_attention_d64_bf16": (C.c_int, [_P, _P, _P, _P, C.POINTER(FaDesc), _P]),
     "u2_sample_f32": (C.c_int, [_P, _P, _I, _I, _L, _F, _I, _F, C.c_uint64, _P, _I, _P]),
     "u2_sample_dev_f32": (C.c_int, [_P, _P, _I, _I, _L, _P, _P, _I, _P]),
+    "u2_logits_process_f32": (C.c_int, [_P, _I, _I, _L, _P, _P, _L, _I, _P, _P, _I, _P]),
     "u2_topk_rows_f32": (C.c_int, [_P, _P, _I, _I, _I, _L, _L, _P]),
     "u2_dlinear_ws_elems": (C.c_int64, [_I, _I]),
     "u2_dlinear_multi_bf16": (C.c_int, [_P, _P, _P, _P, _I, _P, _P, _I, _P, _P]),

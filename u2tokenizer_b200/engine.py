@@ -34,6 +34,22 @@ def _pad8(n: int) -> int:
     return (n + 7) // 8 * 8
 
 
+@dataclass(frozen=True)
+class LogitsProcessors:
+    """HF generate()'s repetition_penalty, no_repeat_ngram_size, bad_words_ids and min_new_tokens, applied by one
+    kernel to every step's logits before the pick (ops.logits_process). The history is the generated tokens only.
+    eos_token_ids: the ids min_new_tokens keeps out. Validated values: see modeling's _generate_logits_processors."""
+    repetition_penalty: float = 1.0
+    no_repeat_ngram_size: int = 0
+    min_new_tokens: int = 0
+    eos_token_ids: Tuple[int, ...] = ()
+    bad_words_ids: Tuple[Tuple[int, ...], ...] = ()
+
+    def neutral(self) -> bool:
+        return (self.repetition_penalty == 1.0 and self.no_repeat_ngram_size == 0 and not self.bad_words_ids
+                and (self.min_new_tokens == 0 or not self.eos_token_ids))
+
+
 class _Take:
     """Pops tensors out of the source state dict (so fused copies do not double peak memory)."""
 
@@ -115,6 +131,9 @@ class U2Engine:
         self._sampling = None
         self._samp_dev = None   # 24-byte u2_sample_params block in device memory (read by the captured decode graph)
         self._samp_host = None
+        self._procs = None      # LogitsProcessors installed for the current generate() call, None when neutral
+        self._lp_dev = None     # its u2_logits_proc_params block in device memory (read by the captured decode graph)
+        self._lp_host = None
 
     # =========================================================================================
     # weight preparation
@@ -693,7 +712,11 @@ class U2Engine:
 
     def _pick_next(self, logits: torch.Tensor, ids_out: torch.Tensor, step_dev: Optional[torch.Tensor], step: int = 0):
         """Greedy argmax, or the sampled head (temperature -> top-k -> top-p -> multinomial) when a sampling
-        configuration is active (HF generate(do_sample=True, ...), reference eval/mrg.py:74-75)."""
+        configuration is active (HF generate(do_sample=True, ...), reference eval/mrg.py:74-75). Installed logits
+        processors rewrite the logits in place first, from the generation state's history of generated tokens."""
+        if self._procs is not None:
+            ops.logits_process(logits, self._procs_block(self._procs), ids_out, self._gen_state["hist"], step=step,
+                               step_dev=step_dev)
         sp = self._sampling
         if sp is None:
             ops.argmax(logits, ids_out)
@@ -712,6 +735,23 @@ class U2Engine:
             ops.sample_params(self.dev, sp["temperature"], sp["top_k"], sp["top_p"], sp["seed"], out=self._samp_dev)
         self._samp_host = cur
         return self._samp_dev
+
+    def _procs_block(self, pc: "LogitsProcessors") -> torch.Tensor:
+        kw = dict(repetition_penalty=pc.repetition_penalty, no_repeat_ngram_size=pc.no_repeat_ngram_size,
+                  min_new_tokens=pc.min_new_tokens, eos_token_ids=pc.eos_token_ids, bad_words_ids=pc.bad_words_ids)
+        if self._lp_dev is None:
+            self._lp_dev = ops.logits_proc_params(self.dev, self.g.vocab_size, **kw)
+        elif self._lp_host != pc:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("logits processors changed inside a CUDA-graph capture")
+            ops.logits_proc_params(self.dev, self.g.vocab_size, out=self._lp_dev, **kw)
+        self._lp_host = pc
+        return self._lp_dev
+
+    @staticmethod
+    def _active(processors: Optional["LogitsProcessors"]) -> Optional["LogitsProcessors"]:
+        """A neutral configuration runs exactly as no configuration: no extra launch, the same captured graph."""
+        return None if processors is None or processors.neutral() else processors
 
     def decode_step(self, cache: "KVCache") -> torch.Tensor:
         """Consumes buffers['ids'] [B,1] (the last token of every sequence), appends sequence b to the cache at
@@ -749,8 +789,10 @@ class U2Engine:
     @torch.no_grad()
     def generate(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id=None, do_sample: bool = False,
                  temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, seed: int = 0, use_graph: bool = True,
-                 num_return_sequences: int = 1, lengths=None):
+                 num_return_sequences: int = 1, lengths=None, processors: Optional[LogitsProcessors] = None):
         """Greedy (do_sample=False) or sampled decoding; same loop, only the token-picking head differs.
+        processors (optional): HF's repetition penalty / no-repeat n-gram / bad words / min new tokens, applied to every
+        step's logits before the pick; every row of a chunk of rows keeps its own history of generated tokens.
         num_return_sequences > 1 (HF semantics: row b * n + s is sample s of prompt b) shares ONE vision + prefill pass:
         the prompt's KV rows are replicated into the decode cache (the reference's DPO-data workflow draws 8 samples per
         study by re-running the whole model per sample, green_refactored/pred_then_green.py:77-83).
@@ -758,6 +800,7 @@ class U2Engine:
         lengths[b] on, as if it ran alone. None = every prompt fills the whole width."""
         self._sampling = dict(temperature=float(temperature), top_k=int(top_k or 0), top_p=float(top_p),
                               seed=int(seed)) if do_sample else None
+        self._procs = self._active(processors)
         try:
             lens = self._row_lengths(lengths, embeds.shape[0], embeds.shape[1])
             if num_return_sequences > 1:
@@ -777,15 +820,20 @@ class U2Engine:
             return torch.cat(outs, dim=0)
         finally:
             self._sampling = None
+            self._procs = None
 
     def _gen_state_for(self, B: int, cap: int):
         """The static KV cache and the captured decode-step graph are kept across calls with the same (batch, capacity,
-        head configuration): capture + instantiation cost ~0.1 s, which would otherwise be paid per request."""
-        key = (B, cap, self.decode_impl, self.multi_op, self.fine_deps, self._sampling is not None)
+        head configuration): capture + instantiation cost ~0.1 s, which would otherwise be paid per request. With logits
+        processors the state also holds the history of generated tokens, int32 [B, cap]."""
+        key = (B, cap, self.decode_impl, self.multi_op, self.fine_deps, self._sampling is not None,
+               self._procs is not None)
         st = self._gen_state if (self._gen_state is not None and self._gen_state["key"] == key) else None
         if st is None:
             self._gen_state = None  # drop the old cache before allocating the new one
             st = dict(key=key, cache=self.new_cache(B, cap), graph=None, n_graph=0)
+            if self._procs is not None:
+                st["hist"] = torch.zeros(B, cap, device=self.dev, dtype=torch.int32)
             self._gen_state = st
         return st
 
@@ -808,16 +856,25 @@ class U2Engine:
 
     def generate_greedy(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id=None,
                         use_graph: bool = True, return_margins: bool = False, force_ids: Optional[torch.Tensor] = None,
-                        logits_out: Optional[list] = None, lengths=None):
+                        logits_out: Optional[list] = None, lengths=None,
+                        processors: Optional[LogitsProcessors] = None):
         """Prefill on `embeds` [B, L, E], then max_new_tokens decode steps (greedy unless a sampling configuration
         was installed by generate()). Returns new ids [B, n] (and the per-step top-1/top-2 logit margins when
-        asked, for margin-aware parity checks).
+        asked, for margin-aware parity checks). processors: as for generate() (None keeps what generate() installed);
+        the margins and logits_out then hold the processed logits.
         force_ids [B, n] (parity tests): teacher forcing - the returned ids are still this engine's own picks, but the
         token fed to the next step is force_ids[:, step], so one near-tie cannot derail the rest of the comparison.
         logits_out: a list that receives a copy of every step's fp32 logits [B, V].
         lengths [B] (optional): prompt b is embeds[b, :lengths[b]]. The prefill runs over the padded width; causal
         attention keeps the real positions exact, and the cache rows from lengths[b] on are overwritten by the decode
         steps before any step reads them."""
+        if processors is not None:
+            prev, self._procs = self._procs, self._active(processors)
+            try:
+                return self.generate_greedy(embeds, max_new_tokens, eos_token_id, use_graph, return_margins, force_ids,
+                                            logits_out, lengths)
+            finally:
+                self._procs = prev
         B, L, _ = embeds.shape
         lens = self._row_lengths(lengths, B, L)
         st = self._gen_state_for(B, L + max_new_tokens)
@@ -830,7 +887,13 @@ class U2Engine:
                                  force_ids=force_ids, logits_out=logits_out)
 
     def _generate_multi(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id, use_graph: bool, n: int,
-                        lengths=None):
+                        lengths=None, processors: Optional[LogitsProcessors] = None):
+        if processors is not None:
+            prev, self._procs = self._procs, self._active(processors)
+            try:
+                return self._generate_multi(embeds, max_new_tokens, eos_token_id, use_graph, n, lengths)
+            finally:
+                self._procs = prev
         B, L, _ = embeds.shape
         lens = self._row_lengths(lengths, B, L)
         pc = self.new_cache(B, L)

@@ -17,11 +17,13 @@ from __future__ import annotations
 from abc import ABC, abstractmethod
 from typing import Any, Dict, List, Optional, Tuple, Union
 
+import numpy as np
 import torch
 import torch.nn as nn
 from transformers import AutoConfig, AutoModelForCausalLM, LlamaForCausalLM, LlamaModel, Qwen3ForCausalLM, Qwen3Model
 from transformers.modeling_outputs import CausalLMOutputWithPast
 
+from . import _lib
 from .configuration import U2LlamaConfig, U2Qwen3Config
 from .geometry import Geometry
 from .synthetic import param_shapes
@@ -325,6 +327,74 @@ class U2MetaForCausalLM(ABC):
         ids = input_ids.gather(1, idx.to(input_ids.device))
         return ids, lens
 
+    @staticmethod
+    def _generate_logits_processors(kwargs: dict, generation_config, prompt_width: int, eos_token_id, vocab_size: int):
+        """generate()'s repetition_penalty, no_repeat_ngram_size, min_new_tokens / min_length and bad_words_ids (popped
+        from `kwargs`, else read from `generation_config`) -> a validated engine.LogitsProcessors, or None when every
+        value is absent or neutral. HF semantics for generate(inputs_embeds=...): the processors see the generated tokens
+        only; min_length counts from the padded prompt width (max(min_length - prompt_width, 0) new tokens) and
+        min_new_tokens takes precedence over it; without an EOS id min_new_tokens has nothing to ban. bad_words_ids is
+        validated as NoBadWordsLogitsProcessor does, and one-token words equal to an EOS id are dropped first."""
+        from .engine import LogitsProcessors
+
+        def opt(name):
+            v = kwargs.pop(name, None)
+            return getattr(generation_config, name, None) if v is None and generation_config is not None else v
+
+        def count(name, v):
+            if v is None:
+                return None
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 0:
+                raise ValueError(f"`{name}` has to be a non-negative integer, but is {v!r}")
+            return int(v)
+
+        pen = opt("repetition_penalty")
+        if pen is not None:
+            if isinstance(pen, bool) or not isinstance(pen, (int, float, np.floating, np.integer)) or not pen > 0:
+                raise ValueError(f"`repetition_penalty` has to be a strictly positive float, but is {pen!r}")
+            pen = float(pen)
+        ngram = count("no_repeat_ngram_size", opt("no_repeat_ngram_size"))
+        min_new = count("min_new_tokens", opt("min_new_tokens"))
+        min_len = count("min_length", opt("min_length"))
+        if min_new is None:
+            min_new = max((min_len or 0) - int(prompt_width), 0)
+        if eos_token_id is None:
+            eos = []
+        elif isinstance(eos_token_id, torch.Tensor):
+            eos = [int(e) for e in eos_token_id.reshape(-1).tolist()]
+        else:
+            eos = [int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])]
+        bad = opt("bad_words_ids")
+        words = ()
+        if bad is not None:
+            if not isinstance(bad, list) or len(bad) == 0:
+                raise ValueError(f"`bad_words_ids` has to be a non-empty list, but is {bad}.")
+            if any(not isinstance(w, list) for w in bad):
+                raise ValueError(f"`bad_words_ids` has to be a list of lists, but is {bad}.")
+            if any(any(not isinstance(x, (int, np.integer)) or x < 0 for x in w) for w in bad):
+                raise ValueError(f"Each list in `bad_words_ids` has to be a list of positive integers, but is {bad}.")
+            kept = dict.fromkeys(tuple(int(x) for x in w) for w in bad if all(w != [e] for e in eos))
+            if not kept:
+                raise ValueError(f"`bad_words_ids` {bad} holds nothing but EOS ids")
+            if any(len(w) == 0 for w in kept):
+                raise ValueError(f"Each word in `bad_words_ids` needs at least one token, but is {bad}.")
+            out = sorted({x for w in kept for x in w if x >= vocab_size})
+            if out:
+                raise ValueError(f"The model vocabulary size is {vocab_size}, but the following tokens were being "
+                                 f"banned: {out}")
+            words = tuple(kept)
+        # an EOS id outside the vocabulary can never be picked: banning it is a no-op, so it is not sent to the kernel
+        eos_in = tuple(dict.fromkeys(e for e in eos if 0 <= e < vocab_size))
+        if min_new and len(eos_in) > _lib.LP_MAX_EOS:
+            raise ValueError(f"min_new_tokens supports at most {_lib.LP_MAX_EOS} EOS ids, got {len(eos_in)}")
+        if len(words) > _lib.LP_MAX_BAD_WORDS or sum(map(len, words)) > _lib.LP_MAX_BAD_TOKENS:
+            raise ValueError(f"bad_words_ids holds at most {_lib.LP_MAX_BAD_WORDS} words of {_lib.LP_MAX_BAD_TOKENS} "
+                             "tokens in all on the CUDA path")
+        pc = LogitsProcessors(repetition_penalty=1.0 if pen is None else pen, no_repeat_ngram_size=ngram or 0,
+                              min_new_tokens=min_new if eos_in else 0, eos_token_ids=eos_in if min_new else (),
+                              bad_words_ids=words)
+        return None if pc.neutral() else pc
+
     # ---- forward / generate shared by the Llama and Qwen3 wrappers (reference u2llama.py:41-138) ----
     def _u2_forward(self, images=None, input_ids=None, labels=None, attention_mask=None, question_ids=None,
                     position_ids=None, past_key_values=None, inputs_embeds=None, use_cache=None,
@@ -454,11 +524,31 @@ class U2MetaForCausalLM(ABC):
         if pad is None and gc is not None:
             pad = gc.pad_token_id
         n_ret = int(opt("num_return_sequences", 1))
+        procs = self._generate_logits_processors(kwargs, gc, L, eos, eng.g.vocab_size)
+        self._check_remaining_generate_kwargs(kwargs)
+        if n_ret > 1 and not do_sample:
+            raise ValueError("num_return_sequences > 1 needs do_sample=True (greedy decoding is deterministic; HF raises too)")
+        ids = eng.generate(inputs_embeds.to(torch.bfloat16), max_new_tokens=max_new, eos_token_id=eos,
+                           do_sample=bool(do_sample), temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
+                           num_return_sequences=n_ret, lengths=lengths, processors=procs)
+        if eos is not None:
+            eos_t = torch.as_tensor(eos if isinstance(eos, (list, tuple)) else [eos], device=ids.device)
+            hit = torch.isin(ids, eos_t)
+            after = (hit.cumsum(dim=1) - hit.long()) > 0  # strictly after the first EOS
+            if pad is None:
+                pad = int(eos_t[0])
+            ids = ids.masked_fill(after, pad)
+            keep = int((~after).any(dim=0).sum())
+            ids = ids[:, :max(keep, 1)]
+        return ids  # new tokens only, like HF generate() on inputs_embeds (reference u2llama.py:123-127)
+
+    @staticmethod
+    def _check_remaining_generate_kwargs(kwargs: dict):
+        """Consumes the generate() kwargs left after the supported ones."""
         # options that would change the generated ids and are not implemented on the CUDA path must not be dropped
         # silently; pure output-format / cache switches are accepted
-        neutral = {"repetition_penalty": 1.0, "no_repeat_ngram_size": 0, "min_new_tokens": 0, "min_length": 0,
-                   "length_penalty": 1.0, "encoder_repetition_penalty": 1.0, "typical_p": 1.0, "epsilon_cutoff": 0.0,
-                   "eta_cutoff": 0.0, "min_p": None, "bad_words_ids": None, "force_words_ids": None,
+        neutral = {"length_penalty": 1.0, "encoder_repetition_penalty": 1.0, "typical_p": 1.0, "epsilon_cutoff": 0.0,
+                   "eta_cutoff": 0.0, "min_p": None, "force_words_ids": None,
                    "suppress_tokens": None, "begin_suppress_tokens": None, "logits_processor": None,
                    "stopping_criteria": None, "prefix_allowed_tokens_fn": None, "penalty_alpha": None,
                    "num_beam_groups": 1, "diversity_penalty": 0.0}
@@ -476,21 +566,6 @@ class U2MetaForCausalLM(ABC):
                     raise NotImplementedError(f"generate({k}=True) is not implemented on the CUDA path")
         if kwargs:
             raise TypeError(f"generate() got unsupported arguments {sorted(kwargs)}")
-        if n_ret > 1 and not do_sample:
-            raise ValueError("num_return_sequences > 1 needs do_sample=True (greedy decoding is deterministic; HF raises too)")
-        ids = eng.generate(inputs_embeds.to(torch.bfloat16), max_new_tokens=max_new, eos_token_id=eos,
-                           do_sample=bool(do_sample), temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
-                           num_return_sequences=n_ret, lengths=lengths)
-        if eos is not None:
-            eos_t = torch.as_tensor(eos if isinstance(eos, (list, tuple)) else [eos], device=ids.device)
-            hit = torch.isin(ids, eos_t)
-            after = (hit.cumsum(dim=1) - hit.long()) > 0  # strictly after the first EOS
-            if pad is None:
-                pad = int(eos_t[0])
-            ids = ids.masked_fill(after, pad)
-            keep = int((~after).any(dim=0).sum())
-            ids = ids[:, :max(keep, 1)]
-        return ids  # new tokens only, like HF generate() on inputs_embeds (reference u2llama.py:123-127)
 
 
 class _U2TrainLoss(torch.autograd.Function):

@@ -568,6 +568,74 @@ def sample_dev(logits: torch.Tensor, params: torch.Tensor, out: Optional[torch.T
     return out
 
 
+def logits_proc_params(device, vocab_size: int, *, repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
+                       min_new_tokens: int = 0, eos_token_ids=(), bad_words_ids=(),
+                       out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The u2_logits_proc_params block (include/u2b200.h) in device memory, as uint8. `out` (a block made earlier) is
+    overwritten in place, so a captured decode graph gets a new request's processors without a new capture.
+    Raises ValueError for values the kernel cannot take (over capacity, token ids outside [0, vocab_size))."""
+    import numpy as np
+    p = float(repetition_penalty)
+    if not p > 0:
+        raise ValueError(f"repetition_penalty must be > 0, got {repetition_penalty}")
+    n, k = int(no_repeat_ngram_size), int(min_new_tokens)
+    if n < 0 or k < 0:
+        raise ValueError("no_repeat_ngram_size and min_new_tokens must be >= 0")
+    eos = [int(e) for e in eos_token_ids]
+    words = [[int(x) for x in w] for w in bad_words_ids]
+    if len(eos) > _lib.LP_MAX_EOS:
+        raise ValueError(f"at most {_lib.LP_MAX_EOS} EOS ids, got {len(eos)}")
+    if len(words) > _lib.LP_MAX_BAD_WORDS or sum(map(len, words)) > _lib.LP_MAX_BAD_TOKENS:
+        raise ValueError(f"bad_words_ids holds at most {_lib.LP_MAX_BAD_WORDS} words of "
+                         f"{_lib.LP_MAX_BAD_TOKENS} tokens in all")
+    if any(len(w) == 0 for w in words):
+        raise ValueError("bad_words_ids: every word needs at least one token")
+    bad = [v for v in eos + [x for w in words for x in w] if not 0 <= v < vocab_size]
+    if bad:
+        raise ValueError(f"token ids {bad} outside the vocabulary [0, {vocab_size})")
+    blk = _lib.LogitsProcParams()
+    blk.penalty = p
+    blk.inv_penalty = float(np.float32(1.0) / np.float32(p))  # fp32 reciprocal of the fp32 penalty, as torch on CUDA
+    blk.ngram, blk.min_new, blk.n_eos, blk.n_bad = n, k, len(eos), len(words)
+    for i, e in enumerate(eos):
+        blk.eos[i] = e
+    off = 0
+    for i, w in enumerate(words):
+        blk.bad_off[i] = off
+        for x in w:
+            blk.bad_tok[off] = x
+            off += 1
+    blk.bad_off[len(words)] = off
+    host = torch.frombuffer(bytearray(bytes(blk)), dtype=torch.uint8)
+    if out is None:
+        return host.to(device)
+    out.copy_(host)
+    return out
+
+
+def logits_process(logits: torch.Tensor, params: torch.Tensor, ids: torch.Tensor, hist: torch.Tensor, *,
+                   step: int = 0, step_dev=None) -> torch.Tensor:
+    """HF's repetition penalty -> no-repeat n-gram -> bad words -> min new tokens, in place on fp32 logits [B, V].
+    ids [B] int64: the token fed to this step, appended to the history hist [B, cap] int32 at column t - 1 where
+    t = *step_dev (or step) is the number of generated tokens. params: a block made by logits_proc_params()."""
+    _need_cuda(logits, params, ids, hist, step_dev)
+    B, V = logits.shape
+    if logits.dtype != F32 or logits.stride(1) != 1:
+        raise TypeError("logits_process: logits must be fp32 with unit column stride")
+    if params.dtype != torch.uint8 or params.numel() != C.sizeof(_lib.LogitsProcParams):
+        raise ValueError("logits_process: params must be the block of logits_proc_params()")
+    if ids.dtype != torch.int64 or ids.numel() != B or not ids.is_contiguous():
+        raise ValueError("logits_process: ids must be contiguous int64 [B]")
+    if hist.dtype != torch.int32 or hist.dim() != 2 or hist.shape[0] != B or hist.stride(1) != 1:
+        raise ValueError("logits_process: hist must be int32 [B, cap] with unit column stride")
+    if step_dev is None and not 0 <= step <= hist.shape[1]:
+        raise ValueError(f"logits_process: step {step} outside the history capacity {hist.shape[1]}")
+    _lib.check(_lib.load().u2_logits_process_f32(logits.data_ptr(), B, V, logits.stride(0), ids.data_ptr(),
+                                                 hist.data_ptr(), hist.stride(0), hist.shape[1], params.data_ptr(),
+                                                 _ptr(step_dev), int(step), _stream()), "u2_logits_process_f32")
+    return logits
+
+
 def lmhead_logprob(hidden: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor, *, want_lse: bool = False,
                    want_logit_sum: bool = False, nll_acc: Optional[torch.Tensor] = None, ws: Optional[torch.Tensor] = None):
     """logp[r] = log_softmax(hidden[r] @ weight.T)[labels[r]] (0 where labels[r] < 0) without materialising the logits.
