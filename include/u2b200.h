@@ -221,11 +221,12 @@ U2_API int u2_rope_bf16(void* x, const u2_rope_desc* desc, void* stream);
  * [B, Hkv, Tmax, dh]; T valid keys (or *T_dev when T_dev != NULL; T_dev[b] for sequence b when T_per_seq != 0,
  * which needs T_dev). Replaces the HF eager attention at q_len == 1
  * (transformers models/qwen3/modeling_qwen3.py:252-291) inside generate() (src/model/language_model/u2llama.py:123-126);
- * unfused variant used by the CUDA-core decode path. */
+ * unfused variant used by the CUDA-core decode path. kv_src (int32 [B, ld_kv_src] or NULL): the beam-indirect cache of
+ * u2_fused_decode_desc, key t < T - 1 of sequence b from cache row kv_src[b * ld_kv_src + t]. */
 U2_API int u2_decode_attention_bf16(const void* q, const void* k_cache, const void* v_cache, void* out,
                                     int32_t B, int32_t Hq, int32_t Hkv, int32_t dh, int32_t Tmax, int32_t T,
                                     const int32_t* T_dev, int64_t ldq, int64_t ldo, float scale, int32_t T_per_seq,
-                                    void* stream);
+                                    const int32_t* kv_src, int64_t ld_kv_src, void* stream);
 
 /* Decode-step linear (weight streaming, HBM-bound): y[b, n] = sum_k norm(x)[b, k] * w[n, k] (+ residual).
  * CUDA-core variant of the HF decoder Linears (+ Qwen3RMSNorm, modeling_qwen3.py:50-67) at q_len == 1 inside generate()
@@ -339,6 +340,10 @@ typedef struct u2_fused_decode_desc {
                           and K/V prefetch overlap the tail of the preceding kernel, which must not write the cache */
   int32_t pos_per_seq; /* != 0: sequence b appends at pos_dev[b] and attends over pos_dev[b] + 1 keys (a batch of
                           prompts of different lengths; needs pos_dev); 0: pos_dev[0] (or pos) for every sequence */
+  const int32_t* kv_src; /* beam-indirect cache: int32 [B, ld_kv_src]; sequence b reads the key / value of position
+                            t < pos from cache row kv_src[b * ld_kv_src + t] (its new token is always appended to and
+                            read from its own row). NULL: every sequence reads its own row (compiled without lookups) */
+  int64_t ld_kv_src;     /* >= Tmax when kv_src != NULL */
 } u2_fused_decode_desc;
 U2_API int u2_decode_attention_fused_bf16(const void* qkv, void* k_cache, void* v_cache, void* out,
                                           const u2_fused_decode_desc* desc, void* stream);
@@ -425,6 +430,68 @@ typedef struct u2_logits_proc_params {
 U2_API int u2_logits_process_f32(float* logits, int32_t B, int32_t V, int64_t ld, const int64_t* ids, int32_t* hist,
                                  int64_t ld_hist, int32_t hist_cap, const u2_logits_proc_params* params_dev,
                                  const int32_t* step_dev, int32_t step, void* stream);
+
+/* Beam search (HF generate(num_beams=K, length_penalty, early_stopping): GenerationMixin._beam_search, transformers
+ * generation/utils.py, with the prompt length 0 of generate(inputs_embeds=...)) inside the captured decode step.
+ * Prompt b owns rows b*K .. b*K+K-1 of the decode batch; row b*K+k is HF's running beam k. One step:
+ *   u2_log_softmax_f32: lp = log_softmax(logits) (fp32, separate buffer; u2_logits_process_f32 may then run on lp);
+ *   u2_beam_topk_f32:   per row, the top C = beams_to_keep of lp[v] + running[row], sorted (score descending, token
+ *                       ascending on ties) into cand_val / cand_tok [rows, U2_BEAM_MAX_KEEP];
+ *   u2_beam_step:       per prompt, the top C of its K*C row candidates (ties: lower beam * V + token), the stopping
+ *                       criteria (token in eos, or t + 1 == max_new_tokens), the next running beams, the finished
+ *                       hypotheses (score logprob_sum / (t+1)^length_penalty, -1e9 masks as HF adds them), the early-stop
+ *                       heuristic and the prompt's done flag. A done prompt is frozen: later steps change nothing of it.
+ * t = *step_dev (or step) = tokens generated before this step's. State (device memory, set up by the caller):
+ *   running [rows]          running beam scores, {0, -1e9, ...} per prompt at t = 0
+ *   fin_score [rows]        finished hypotheses per prompt, best first, -1e9 at t = 0
+ *   fin_info [rows][4]      (is finished, step t of its last token or -1, parent beam, last token), (0, -1, 0, 0) at t = 0
+ *   flags [prompts][2]      (early-stop heuristic unsatisfied, done), (1, 0) at t = 0
+ *   ids [rows] int64        the next token of every row (the decode step's input)
+ *   rec [rec_rows][rows][2] (token, parent beam) of every running row after step t: the output is backtracked from it
+ *   kv_src [rows, ld_kv_src] the cache indirection of u2_fused_decode_desc: row k of prompt b takes row parent_k's
+ *                           entries at the positions that hold K/V (pos_dev[b*K] + 1 of them after a decode step, pos_dev[b*K]
+ *                           at t = 0) and its own row at the next position
+ *   hist [rows, ld_hist]    optional: the u2_logits_process_f32 history, first t columns reordered like kv_src.
+ * Parameters in DEVICE memory, so a captured step picks up a new request's values; the caller validates them. */
+#define U2_BEAM_MAX_BEAMS 16
+#define U2_BEAM_MAX_EOS 8
+#define U2_BEAM_MAX_KEEP 144 /* max(2, 1 + n_eos) * num_beams */
+typedef struct u2_beam_params {
+  double length_penalty;
+  int32_t num_beams;       /* K, 2..U2_BEAM_MAX_BEAMS */
+  int32_t beams_to_keep;   /* max(2, 1 + n_eos) * K */
+  int32_t early_stopping;  /* 0: False (heuristic), 1: True, 2: "never" */
+  int32_t max_new_tokens;
+  int32_t n_eos;
+  int32_t reserved;
+  int32_t eos[U2_BEAM_MAX_EOS];
+} u2_beam_params;
+typedef struct u2_beam_step_desc {
+  const u2_beam_params* params;
+  int32_t prompts, V;
+  const float* cand_val;
+  const int32_t* cand_tok;
+  float* running;
+  float* fin_score;
+  int32_t* fin_info;
+  int32_t* flags;
+  int64_t* ids;
+  int32_t* rec;
+  int64_t ld_rec;
+  int32_t rec_rows;
+  int32_t* kv_src;
+  int64_t ld_kv_src;
+  const int32_t* pos_dev;
+  int32_t* hist;
+  int64_t ld_hist;
+  int32_t hist_cap;
+  const int32_t* step_dev;
+} u2_beam_step_desc;
+U2_API int u2_log_softmax_f32(const float* x, float* y, int32_t rows, int32_t V, int64_t ldx, int64_t ldy, void* stream);
+U2_API int u2_beam_topk_f32(const float* logprobs, int64_t ld, int32_t rows, int32_t V, const float* running,
+                            const int32_t* flags, const u2_beam_params* params_dev, float* cand_val, int32_t* cand_tok,
+                            void* stream);
+U2_API int u2_beam_step(const u2_beam_step_desc* desc, int32_t step, void* stream);
 
 /* Fused lm_head + selective log-softmax (the DPO / SFT log-probability head) -----------------------------------
  * logp[r] = log_softmax(hidden[r] . W^T)[labels[r]]  (0 where labels[r] < 0) without materialising the [R, V] logits:

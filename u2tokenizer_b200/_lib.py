@@ -115,6 +115,7 @@ class FusedDecodeDesc(C.Structure):
         ("scale", C.c_float),
         ("kv_splits", C.c_int32), ("pdl", C.c_int32),
         ("pos_per_seq", C.c_int32),
+        ("kv_src", C.c_void_p), ("ld_kv_src", C.c_int64),
     ]
 
 
@@ -204,6 +205,35 @@ class LogitsProcParams(C.Structure):
     ]
 
 
+BEAM_MAX_BEAMS, BEAM_MAX_EOS, BEAM_MAX_KEEP = 16, 8, 144  # U2_BEAM_MAX_* of include/u2b200.h
+
+
+class BeamParams(C.Structure):
+    """Mirror of ``u2_beam_params`` (copied to device memory as raw bytes)."""
+    _fields_ = [
+        ("length_penalty", C.c_double),
+        ("num_beams", C.c_int32), ("beams_to_keep", C.c_int32), ("early_stopping", C.c_int32),
+        ("max_new_tokens", C.c_int32), ("n_eos", C.c_int32), ("reserved", C.c_int32),
+        ("eos", C.c_int32 * BEAM_MAX_EOS),
+    ]
+
+
+class BeamStepDesc(C.Structure):
+    """Mirror of ``u2_beam_step_desc``."""
+    _fields_ = [
+        ("params", C.c_void_p),
+        ("prompts", C.c_int32), ("V", C.c_int32),
+        ("cand_val", C.c_void_p), ("cand_tok", C.c_void_p),
+        ("running", C.c_void_p), ("fin_score", C.c_void_p), ("fin_info", C.c_void_p), ("flags", C.c_void_p),
+        ("ids", C.c_void_p),
+        ("rec", C.c_void_p), ("ld_rec", C.c_int64), ("rec_rows", C.c_int32),
+        ("kv_src", C.c_void_p), ("ld_kv_src", C.c_int64),
+        ("pos_dev", C.c_void_p),
+        ("hist", C.c_void_p), ("ld_hist", C.c_int64), ("hist_cap", C.c_int32),
+        ("step_dev", C.c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/u2b200.h / u2b200_train.h declares must be listed here
 # (tests/test_abi.py cross-checks this table against the header and the built library).
 _P, _I, _L, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
@@ -227,7 +257,7 @@ SIGNATURES = {
     "u2_embed_splice_bf16": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _L, _P]),
     "u2_temporal_attention_bf16": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _L, _L, _F, _P, _I, _P]),
     "u2_rope_bf16": (C.c_int, [_P, C.POINTER(RopeDesc), _P]),
-    "u2_decode_attention_bf16": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _L, _L, _F, _I, _P]),
+    "u2_decode_attention_bf16": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _L, _L, _F, _I, _P, _L, _P]),
     "u2_gemv_bf16": (C.c_int, [_P, _P, _P, C.POINTER(GemvDesc), _P]),
     "u2_argmax_f32": (C.c_int, [_P, _P, _P, _I, _I, _L, _P]),
     "u2_dlinear_bf16": (C.c_int, [_P, _P, _P, C.POINTER(DlinearDesc), _P]),
@@ -238,6 +268,9 @@ SIGNATURES = {
     "u2_sample_dev_f32": (C.c_int, [_P, _P, _I, _I, _L, _P, _P, _I, _P]),
     "u2_logits_process_f32": (C.c_int, [_P, _I, _I, _L, _P, _P, _L, _I, _P, _P, _I, _P]),
     "u2_topk_rows_f32": (C.c_int, [_P, _P, _I, _I, _I, _L, _L, _P]),
+    "u2_log_softmax_f32": (C.c_int, [_P, _P, _I, _I, _L, _L, _P]),
+    "u2_beam_topk_f32": (C.c_int, [_P, _L, _I, _I, _P, _P, _P, _P, _P, _P]),
+    "u2_beam_step": (C.c_int, [C.POINTER(BeamStepDesc), _I, _P]),
     "u2_dlinear_ws_elems": (C.c_int64, [_I, _I]),
     "u2_dlinear_multi_bf16": (C.c_int, [_P, _P, _P, _P, _I, _P, _P, _I, _P, _P]),
     "u2_preprocess_ws_bytes": (C.c_int64, [_I, _I, _I]),

@@ -8,6 +8,8 @@
 #include <cuda_bf16.h>
 #include <math.h>
 
+#include <type_traits>
+
 #include "host_util.h"
 #include "u2b200.h"
 
@@ -202,12 +204,26 @@ __device__ __forceinline__ void load_epl(const __nv_bfloat16* p, float (&f)[kEpl
   }
 }
 
-template <int kEpl>  // dh = kEpl * 32: lane owns elements [lane*kEpl, lane*kEpl + kEpl)
+// Beam-indirect cache (kInd): sequence b reads the key / value of position t from cache row kv_src[b * ld_src + t]
+// (FasterTransformer's "cache indirection"); its own newest position (t == pos) always comes from row b. Returns the
+// element offset from row b's slot to the source row's slot. kInd == false compiles to nothing.
+template <bool kInd>
+__device__ __forceinline__ long long kv_src_delta(const int* __restrict__ kv_src, long long ld_src, int b, int t,
+                                                  int pos, long long row_elems) {
+  if constexpr (kInd) {
+    const int r = t == pos ? b : __ldg(kv_src + (long long)b * ld_src + t);
+    return (long long)(r - b) * row_elems;
+  } else {
+    return 0;
+  }
+}
+
+template <int kEpl, bool kInd>  // dh = kEpl * 32: lane owns elements [lane*kEpl, lane*kEpl + kEpl)
 __global__ void __launch_bounds__(256)
 decode_attention_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
                         const __nv_bfloat16* __restrict__ vc, __nv_bfloat16* __restrict__ out, int Hq, int Hkv,
                         int Tmax, int T_host, const int* __restrict__ T_dev, long long ldq, long long ldo,
-                        float scale, int T_per_seq) {
+                        float scale, int T_per_seq, const int* __restrict__ kv_src, long long ld_src) {
   constexpr int dh = kEpl * 32;
   const int h = blockIdx.x, b = blockIdx.y;
   const int T = T_dev ? min(T_dev[T_per_seq ? b : 0], Tmax) : T_host;
@@ -226,8 +242,9 @@ decode_attention_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16
   for (int i = 0; i < kEpl; ++i) acc[i] = 0.f;
   for (int t = warp; t < T; t += 8) {
     float kk[kEpl], vv[kEpl];
-    load_epl<kEpl>(kp + (long long)t * dh, kk);
-    load_epl<kEpl>(vp + (long long)t * dh, vv);
+    const long long off = (long long)t * dh + kv_src_delta<kInd>(kv_src, ld_src, b, t, T - 1, (long long)Hkv * Tmax * dh);
+    load_epl<kEpl>(kp + off, kk);
+    load_epl<kEpl>(vp + off, vv);
     float d = 0.f;
 #pragma unroll
     for (int i = 0; i < kEpl; ++i) d += qv[i] * kk[i];
@@ -323,19 +340,23 @@ extern "C" U2_API int u2_rope_bf16(void* x, const u2_rope_desc* d, void* stream)
 extern "C" U2_API int u2_decode_attention_bf16(const void* q, const void* k_cache, const void* v_cache, void* out,
                                                int32_t B, int32_t Hq, int32_t Hkv, int32_t dh, int32_t Tmax,
                                                int32_t T, const int32_t* T_dev, int64_t ldq, int64_t ldo,
-                                               float scale, int32_t T_per_seq, void* stream) {
+                                               float scale, int32_t T_per_seq, const int32_t* kv_src,
+                                               int64_t ld_kv_src, void* stream) {
   if (!q || !k_cache || !v_cache || !out) return set_error(U2_ERR_ARG, "decode_attention: null pointer");
   if (Hkv <= 0 || Hq % Hkv) return set_error(U2_ERR_ARG, "decode_attention: Hq must be a multiple of Hkv");
   if (!T_dev && (T <= 0 || T > Tmax)) return set_error(U2_ERR_ARG, "decode_attention: need 0 < T <= Tmax");
   if (T_per_seq && !T_dev) return set_error(U2_ERR_ARG, "decode_attention: T_per_seq needs T_dev");
+  if (kv_src && ld_kv_src < Tmax) return set_error(U2_ERR_ARG, "decode_attention: kv_src row stride < Tmax");
   dim3 grid((unsigned)Hq, (unsigned)B);
-#define U2_DA(EPL) decode_attention_kernel<EPL><<<grid, 256, 0, ST(stream)>>>(CBF(q), CBF(k_cache), CBF(v_cache), BF(out), Hq, Hkv, Tmax, T, T_dev, ldq, ldo, scale, T_per_seq != 0)
+#define U2_DA(EPL, IND) decode_attention_kernel<EPL, IND><<<grid, 256, 0, ST(stream)>>>(CBF(q), CBF(k_cache), CBF(v_cache), BF(out), Hq, Hkv, Tmax, T, T_dev, ldq, ldo, scale, T_per_seq != 0, kv_src, ld_kv_src)
+#define U2_DA2(EPL) if (kv_src) U2_DA(EPL, true); else U2_DA(EPL, false)
   switch (dh) {
-    case 32: U2_DA(1); break;
-    case 64: U2_DA(2); break;
-    case 128: U2_DA(4); break;
+    case 32: U2_DA2(1); break;
+    case 64: U2_DA2(2); break;
+    case 128: U2_DA2(4); break;
     default: return set_error(U2_ERR_UNSUPPORTED, "decode_attention: head_dim %d (supported: 32, 64, 128)", dh);
   }
+#undef U2_DA2
 #undef U2_DA
   U2_CHECK_LAUNCH("decode_attention");
   return U2_OK;
@@ -375,6 +396,19 @@ struct FusedDecodeArgs {
   const float* inv_freq;     // [dh/2]
   float scale;
 };
+// beam search: the cache row of every position, int32 [B, ld_src]. A separate type, so that the kernels without the
+// table keep the parameter block (and the code) they had before it existed
+struct FusedDecodeIndArgs : FusedDecodeArgs {
+  const int* kv_src;
+  long long ld_src;
+};
+template <bool kInd>
+using FusedArgsT = std::conditional_t<kInd, FusedDecodeIndArgs, FusedDecodeArgs>;
+template <bool kInd>
+__device__ __forceinline__ long long kv_src_delta(const FusedArgsT<kInd>& a, int b, int t, int pos, long long row_elems) {
+  if constexpr (kInd) return kv_src_delta<true>(a.kv_src, a.ld_src, b, t, pos, row_elems);
+  else return 0;
+}
 
 template <int kDh>
 __device__ __forceinline__ void norm_rope_head(const __nv_bfloat16* src, const float* nw, float eps,
@@ -414,9 +448,9 @@ __device__ __forceinline__ void norm_rope_head(const __nv_bfloat16* src, const f
   }
 }
 
-template <int kDh, int kG>
+template <int kDh, int kG, bool kInd>
 __global__ void __launch_bounds__(FaCfg<kDh, kG>::kWarps * 32)
-fused_decode_attention_kernel(const FusedDecodeArgs a) {
+fused_decode_attention_kernel(const FusedArgsT<kInd> a) {
   constexpr int kFaWarps = FaCfg<kDh, kG>::kWarps;
   constexpr int kEpl = kDh / 32;  // head_dim elements per lane in the PV phase
   constexpr int kPf = 16;         // V rows prefetched per batch (memory-level parallelism in the PV loop)
@@ -458,13 +492,16 @@ fused_decode_attention_kernel(const FusedDecodeArgs a) {
 #pragma unroll
     for (int i = 0; i < kEpl; ++i) acc[g][i] = 0.f;
   }
+  const long long row_elems = (long long)a.Hkv * a.Tmax * kDh;
   for (int t0 = warp * 32; t0 < T; t0 += kFaWarps * 32) {
     const int t = t0 + lane;
+    // lane's key row (clamped like the V rows below); the V loop takes the other lanes' offsets by shuffle
+    const long long dsrc = kv_src_delta<kInd>(a, b, min(t, T - 1), pos, row_elems);
     float s[kG];
 #pragma unroll
     for (int g = 0; g < kG; ++g) s[g] = 0.f;
     if (t < T) {
-      const uint4* kr = reinterpret_cast<const uint4*>(kbase + (long long)t * kDh);
+      const uint4* kr = reinterpret_cast<const uint4*>(kbase + (long long)t * kDh + dsrc);
       // the whole K row of this lane's key in one burst of independent 16-byte loads (one L2 round trip)
       uint4 u[kDh / 8];
 #pragma unroll
@@ -511,7 +548,9 @@ fused_decode_attention_kernel(const FusedDecodeArgs a) {
 #pragma unroll
       for (int jj = 0; jj < kPf; ++jj) {
         const int tj = min(t0 + j0 + jj, T - 1);  // clamped rows carry probability 0
-        load_epl<kEpl>(vbase + (long long)tj * kDh + lane * kEpl, vv[jj]);
+        long long dj = 0;
+        if constexpr (kInd) dj = __shfl_sync(0xffffffffu, dsrc, tj - t0);
+        load_epl<kEpl>(vbase + (long long)tj * kDh + dj + lane * kEpl, vv[jj]);
       }
 #pragma unroll
       for (int jj = 0; jj < kPf; ++jj) {
@@ -561,9 +600,9 @@ fused_decode_attention_kernel(const FusedDecodeArgs a) {
 // k / v never go through global memory (every CTA recomputes them into shared memory, rank 0 appends them to the
 // cache). CTA partials (m, l, o) are merged by rank 0 over distributed shared memory.
 // ------------------------------------------------------------------------------------------------
-template <int kDh, int kG>
+template <int kDh, int kG, bool kInd>
 __global__ void __launch_bounds__(256)
-fused_decode_attention_split_kernel(const FusedDecodeArgs a) {
+fused_decode_attention_split_kernel(const FusedArgsT<kInd> a) {
   namespace cg = cooperative_groups;
   cg::cluster_group cluster = cg::this_cluster();
   constexpr int kW = 8;
@@ -591,19 +630,24 @@ fused_decode_attention_split_kernel(const FusedDecodeArgs a) {
   __nv_bfloat16* kbase = a.kc + ((long long)b * a.Hkv + hk) * a.Tmax * kDh;
   __nv_bfloat16* vbase = a.vc + ((long long)b * a.Hkv + hk) * a.Tmax * kDh;
 
-  // ---- request this warp's first key group (rows >= pos are stale: they are replaced from shared memory below)
+  // ---- request this warp's first key group (rows >= pos are stale: they are replaced from shared memory below).
+  // A beam-indirection table is written by the previous step's beam kernel, like the positions: safe to read here
   uint4 ku[kDh / 8];
   uint32_t vw[32][kVw];
   int t0 = (warp * S + rank) * 32;
+  const long long row_elems = (long long)a.Hkv * a.Tmax * kDh;
   auto request = [&](int base) {
     const int t = min(base + lane, T - 1);
-    const uint4* kr = reinterpret_cast<const uint4*>(kbase + (long long)t * kDh);
+    const long long dsrc = kv_src_delta<kInd>(a, b, t, pos, row_elems);
+    const uint4* kr = reinterpret_cast<const uint4*>(kbase + (long long)t * kDh + dsrc);
 #pragma unroll
     for (int c = 0; c < kDh / 8; ++c) ku[c] = kr[c];
 #pragma unroll
     for (int jj = 0; jj < 32; ++jj) {
       const int tj = min(base + jj, T - 1);
-      const __nv_bfloat16* vp = vbase + (long long)tj * kDh + lane * kEpl;
+      long long dj = 0;
+      if constexpr (kInd) dj = __shfl_sync(0xffffffffu, dsrc, tj - base);
+      const __nv_bfloat16* vp = vbase + (long long)tj * kDh + dj + lane * kEpl;
       if constexpr (kEpl == 4) {
         const uint2 u = *reinterpret_cast<const uint2*>(vp);
         vw[jj][0] = u.x;
@@ -767,8 +811,8 @@ fused_decode_attention_split_kernel(const FusedDecodeArgs a) {
   cluster.sync();  // the other ranks' shared memory must outlive rank 0's reads
 }
 
-template <int kDh, int kG>
-static int launch_fused_decode_split(const FusedDecodeArgs& a, dim3 grid, bool pdl, cudaStream_t st) {
+template <int kDh, int kG, bool kInd>
+static int launch_fused_decode_split(const FusedArgsT<kInd>& a, dim3 grid, bool pdl, cudaStream_t st) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = dim3(256);
@@ -783,30 +827,36 @@ static int launch_fused_decode_split(const FusedDecodeArgs& a, dim3 grid, bool p
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 2 : 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, fused_decode_attention_split_kernel<kDh, kG>, a);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, fused_decode_attention_split_kernel<kDh, kG, kInd>, a);
   if (e != cudaSuccess) return set_error(U2_ERR_CUDA, "decode_attention_fused (split-KV) launch: %s", cudaGetErrorString(e));
   return U2_OK;
 }
 
-template <int kDh>
-static int launch_fused_decode(const FusedDecodeArgs& a, int G, dim3 grid, bool pdl, cudaStream_t st) {
+template <int kDh, bool kInd>
+static int launch_fused_decode(const FusedArgsT<kInd>& a, int G, dim3 grid, bool pdl, cudaStream_t st) {
   if (grid.z > 1) {
     switch (G) {
-      case 1: return launch_fused_decode_split<kDh, 1>(a, grid, pdl, st);
-      case 2: return launch_fused_decode_split<kDh, 2>(a, grid, pdl, st);
-      case 4: return launch_fused_decode_split<kDh, 4>(a, grid, pdl, st);
-      case 8: return launch_fused_decode_split<kDh, 8>(a, grid, pdl, st);
+      case 1: return launch_fused_decode_split<kDh, 1, kInd>(a, grid, pdl, st);
+      case 2: return launch_fused_decode_split<kDh, 2, kInd>(a, grid, pdl, st);
+      case 4: return launch_fused_decode_split<kDh, 4, kInd>(a, grid, pdl, st);
+      case 8: return launch_fused_decode_split<kDh, 8, kInd>(a, grid, pdl, st);
       default: return set_error(U2_ERR_UNSUPPORTED, "decode_attention_fused: Hq/Hkv = %d (supported 1, 2, 4, 8)", G);
     }
   }
   switch (G) {
-    case 1: fused_decode_attention_kernel<kDh, 1><<<grid, FaCfg<kDh, 1>::kWarps * 32, 0, st>>>(a); break;
-    case 2: fused_decode_attention_kernel<kDh, 2><<<grid, FaCfg<kDh, 2>::kWarps * 32, 0, st>>>(a); break;
-    case 4: fused_decode_attention_kernel<kDh, 4><<<grid, FaCfg<kDh, 4>::kWarps * 32, 0, st>>>(a); break;
-    case 8: fused_decode_attention_kernel<kDh, 8><<<grid, FaCfg<kDh, 8>::kWarps * 32, 0, st>>>(a); break;
+    case 1: fused_decode_attention_kernel<kDh, 1, kInd><<<grid, FaCfg<kDh, 1>::kWarps * 32, 0, st>>>(a); break;
+    case 2: fused_decode_attention_kernel<kDh, 2, kInd><<<grid, FaCfg<kDh, 2>::kWarps * 32, 0, st>>>(a); break;
+    case 4: fused_decode_attention_kernel<kDh, 4, kInd><<<grid, FaCfg<kDh, 4>::kWarps * 32, 0, st>>>(a); break;
+    case 8: fused_decode_attention_kernel<kDh, 8, kInd><<<grid, FaCfg<kDh, 8>::kWarps * 32, 0, st>>>(a); break;
     default: return set_error(U2_ERR_UNSUPPORTED, "decode_attention_fused: Hq/Hkv = %d (supported 1, 2, 4, 8)", G);
   }
   return U2_OK;
+}
+
+template <int kDh>
+static int launch_fused_decode(const FusedDecodeIndArgs& a, int G, dim3 grid, bool pdl, cudaStream_t st) {
+  if (a.kv_src) return launch_fused_decode<kDh, true>(a, G, grid, pdl, st);
+  return launch_fused_decode<kDh, false>(static_cast<const FusedDecodeArgs&>(a), G, grid, pdl, st);
 }
 
 }  // namespace u2
@@ -819,7 +869,7 @@ extern "C" U2_API int u2_decode_attention_fused_bf16(const void* qkv, void* k_ca
     return set_error(U2_ERR_UNSUPPORTED, "decode_attention_fused: Hq/Hkv must be an integer <= %d", kFaMaxG);
   if (!d->pos_dev && (d->pos < 0 || d->pos >= d->Tmax)) return set_error(U2_ERR_ARG, "decode_attention_fused: position outside the cache");
   if (d->pos_per_seq && !d->pos_dev) return set_error(U2_ERR_ARG, "decode_attention_fused: pos_per_seq needs pos_dev");
-  FusedDecodeArgs a;
+  FusedDecodeIndArgs a;
   a.qkv = CBF(qkv); a.ldq = d->ldq;
   a.kc = BF(k_cache); a.vc = BF(v_cache);
   a.out = BF(out); a.ldo = d->ldo;
@@ -827,6 +877,8 @@ extern "C" U2_API int u2_decode_attention_fused_bf16(const void* qkv, void* k_ca
   a.pos_dev = d->pos_dev; a.pos_per_seq = d->pos_per_seq != 0; a.pos_host = d->pos;
   a.q_norm_w = d->q_norm_w; a.k_norm_w = d->k_norm_w; a.eps = d->eps;
   a.inv_freq = d->inv_freq; a.scale = d->scale;
+  a.kv_src = d->kv_src; a.ld_src = d->ld_kv_src;
+  if (a.kv_src && a.ld_src < d->Tmax) return set_error(U2_ERR_ARG, "decode_attention_fused: kv_src row stride < Tmax");
   const int splits = d->kv_splits > 1 ? d->kv_splits : 1;
   if (splits != 1 && splits != 2 && splits != 4 && splits != 8)
     return set_error(U2_ERR_ARG, "decode_attention_fused: kv_splits must be 0/1, 2, 4 or 8 (portable cluster sizes)");

@@ -23,7 +23,7 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from . import ops
+from . import _lib, ops
 from .geometry import Geometry
 
 BF16, F32 = torch.bfloat16, torch.float32
@@ -48,6 +48,21 @@ class LogitsProcessors:
     def neutral(self) -> bool:
         return (self.repetition_penalty == 1.0 and self.no_repeat_ngram_size == 0 and not self.bad_words_ids
                 and (self.min_new_tokens == 0 or not self.eos_token_ids))
+
+
+@dataclass(frozen=True)
+class BeamSearch:
+    """HF generate(num_beams, length_penalty, early_stopping, num_return_sequences) on the CUDA path (GenerationMixin.
+    _beam_search): the beams of prompt b are rows b*K .. b*K+K-1 of one decode batch, they continue each other's KV cache
+    through an indirection table, and the per-step selection and bookkeeping run inside the captured decode step
+    (ops.beam_topk / ops.beam_step). early_stopping: True, False or "never". pad_token_id: fills the rows shorter than the
+    longest returned hypothesis (HF's `pad_token_id or eos_token_id[0]`). Validated values: see modeling's
+    _generate_beam_search."""
+    num_beams: int
+    length_penalty: float = 1.0
+    early_stopping: object = False
+    num_return_sequences: int = 1
+    pad_token_id: Optional[int] = None
 
 
 class _Take:
@@ -134,6 +149,10 @@ class U2Engine:
         self._procs = None      # LogitsProcessors installed for the current generate() call, None when neutral
         self._lp_dev = None     # its u2_logits_proc_params block in device memory (read by the captured decode graph)
         self._lp_host = None
+        self._beam = None       # BeamSearch of the current generate() call (num_beams > 1), else None
+        self._beam_dev = None   # its u2_beam_params block in device memory (read by the captured decode graph)
+        self._beam_host = None
+        self.last_beam_scores = None  # fp32 [rows] scores of the hypotheses the last beam search returned
 
     # =========================================================================================
     # weight preparation
@@ -682,7 +701,7 @@ class U2Engine:
             ops.decode_attention_fused(qkv, cache.k[li], cache.v[li], ctx, B=B, Hq=hq, Hkv=hkv, dh=dh, Tmax=cache.max_len,
                                        inv_freq=self.inv_freq, scale=1.0 / math.sqrt(dh), pos_dev=cache.length_dev,
                                        q_norm_w=w["qn"], k_norm_w=w["kn"], eps=eps, kv_splits=self._kv_splits(B),
-                                       pdl=self.pdl and self.attn_pdl, pos_per_seq=True)
+                                       pdl=self.pdl and self.attn_pdl, pos_per_seq=True, kv_src=cache.kv_src)
             last = li + 1 == nl
             g_next = self.final_norm if last else self.layers[li + 1]["ln1"]
             fl = flags[li] if (self.multi_op and self.fine_deps) else [None] * 4
@@ -713,7 +732,10 @@ class U2Engine:
     def _pick_next(self, logits: torch.Tensor, ids_out: torch.Tensor, step_dev: Optional[torch.Tensor], step: int = 0):
         """Greedy argmax, or the sampled head (temperature -> top-k -> top-p -> multinomial) when a sampling
         configuration is active (HF generate(do_sample=True, ...), reference eval/mrg.py:74-75). Installed logits
-        processors rewrite the logits in place first, from the generation state's history of generated tokens."""
+        processors rewrite the logits in place first, from the generation state's history of generated tokens.
+        Beam search replaces all of it with the beam step (_beam_pick)."""
+        if self._beam is not None:
+            return self._beam_pick(logits, ids_out, step_dev, step)
         if self._procs is not None:
             ops.logits_process(logits, self._procs_block(self._procs), ids_out, self._gen_state["hist"], step=step,
                                step_dev=step_dev)
@@ -748,6 +770,34 @@ class U2Engine:
         self._lp_host = pc
         return self._lp_dev
 
+    def _beam_pick(self, logits: torch.Tensor, ids_out: torch.Tensor, step_dev: Optional[torch.Tensor], step: int):
+        """HF's beam step: log_softmax -> logits processors (on the log-probs) -> per-row top beams_to_keep of
+        log-prob + running score -> per-prompt merge and bookkeeping, which also writes the next ids and reorders the
+        cache indirection table and the processor history. logits keeps the raw logits."""
+        st = self._gen_state
+        bs = st["beam"]
+        blk = self._beam_block()
+        lp = ops.log_softmax(logits, bs["lp"])
+        if self._procs is not None:
+            ops.logits_process(lp, self._procs_block(self._procs), ids_out, st["hist"], step=step, step_dev=step_dev)
+        ops.beam_topk(lp, bs["running"], bs["flags"], blk, bs["cand_val"], bs["cand_tok"])
+        ops.beam_step(blk, bs, ids_out, st["cache"].kv_src, st["cache"].length_dev, V=logits.shape[1],
+                      hist=st.get("hist"), step=step, step_dev=step_dev)
+
+    def _beam_block(self) -> torch.Tensor:
+        bm, (max_new, eos) = self._beam, self._beam_req
+        cur = (bm.num_beams, float(bm.length_penalty), bm.early_stopping, max_new, eos)
+        kw = dict(num_beams=bm.num_beams, length_penalty=bm.length_penalty, early_stopping=bm.early_stopping,
+                  max_new_tokens=max_new, eos_token_ids=eos)
+        if self._beam_dev is None:
+            self._beam_dev = ops.beam_params(self.dev, **kw)
+        elif self._beam_host != cur:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("beam search parameters changed inside a CUDA-graph capture")
+            ops.beam_params(self.dev, out=self._beam_dev, **kw)
+        self._beam_host = cur
+        return self._beam_dev
+
     @staticmethod
     def _active(processors: Optional["LogitsProcessors"]) -> Optional["LogitsProcessors"]:
         """A neutral configuration runs exactly as no configuration: no extra launch, the same captured graph."""
@@ -773,7 +823,7 @@ class U2Engine:
                      k_cache=cache.k[li], v_cache=cache.v[li], Tmax=cache.max_len, rows_per_batch=1, pos0_per_batch=True)
             ops.decode_attention(qkv, cache.k[li], cache.v[li], ctx, B=B, Hq=hq, Hkv=hkv, dh=dh, Tmax=cache.max_len,
                                  T_dev=cache.length_plus1_dev, ldq=nqkv, ldo=hq * dh, scale=1.0 / math.sqrt(dh),
-                                 T_per_seq=True)
+                                 T_per_seq=True, kv_src=cache.kv_src)
             ops.gemv(ctx, w["wo"], x, residual=x)
             ops.gemv(x, w["wgu"], act, norm_gamma=w["ln2"], norm_eps=g.rms_norm_eps, silu_pair=True)
             ops.gemv(act, w["wdown"], x, residual=x)
@@ -789,7 +839,8 @@ class U2Engine:
     @torch.no_grad()
     def generate(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id=None, do_sample: bool = False,
                  temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, seed: int = 0, use_graph: bool = True,
-                 num_return_sequences: int = 1, lengths=None, processors: Optional[LogitsProcessors] = None):
+                 num_return_sequences: int = 1, lengths=None, processors: Optional[LogitsProcessors] = None,
+                 beam: Optional[BeamSearch] = None):
         """Greedy (do_sample=False) or sampled decoding; same loop, only the token-picking head differs.
         processors (optional): HF's repetition penalty / no-repeat n-gram / bad words / min new tokens, applied to every
         step's logits before the pick; every row of a chunk of rows keeps its own history of generated tokens.
@@ -797,7 +848,17 @@ class U2Engine:
         the prompt's KV rows are replicated into the decode cache (the reference's DPO-data workflow draws 8 samples per
         study by re-running the whole model per sample, green_refactored/pred_then_green.py:77-83).
         lengths [B] (optional): prompt b is embeds[b, :lengths[b]] (right padding after it); it decodes from position
-        lengths[b] on, as if it ran alone. None = every prompt fills the whole width."""
+        lengths[b] on, as if it ran alone. None = every prompt fills the whole width.
+        beam (num_beams > 1): HF beam search instead of the greedy / sampled pick (do_sample and num_return_sequences are
+        then ignored; the beam config carries its own num_return_sequences)."""
+        if beam is not None and beam.num_beams > 1:
+            self._sampling = None  # the state key must not carry a previous sampled request's flag
+            self._procs = self._active(processors)
+            try:
+                return self._generate_beam(embeds, max_new_tokens, eos_token_id, use_graph, beam,
+                                           self._row_lengths(lengths, embeds.shape[0], embeds.shape[1]))
+            finally:
+                self._procs = None
         self._sampling = dict(temperature=float(temperature), top_k=int(top_k or 0), top_p=float(top_p),
                               seed=int(seed)) if do_sample else None
         self._procs = self._active(processors)
@@ -825,15 +886,28 @@ class U2Engine:
     def _gen_state_for(self, B: int, cap: int):
         """The static KV cache and the captured decode-step graph are kept across calls with the same (batch, capacity,
         head configuration): capture + instantiation cost ~0.1 s, which would otherwise be paid per request. With logits
-        processors the state also holds the history of generated tokens, int32 [B, cap]."""
+        processors the state also holds the history of generated tokens, int32 [B, cap]; with beam search (K > 1) the
+        cache's indirection table and the beam buffers of ops.beam_step."""
+        K = self._beam.num_beams if self._beam is not None else 1
         key = (B, cap, self.decode_impl, self.multi_op, self.fine_deps, self._sampling is not None,
-               self._procs is not None)
+               self._procs is not None, K)
         st = self._gen_state if (self._gen_state is not None and self._gen_state["key"] == key) else None
         if st is None:
             self._gen_state = None  # drop the old cache before allocating the new one
             st = dict(key=key, cache=self.new_cache(B, cap), graph=None, n_graph=0)
             if self._procs is not None:
                 st["hist"] = torch.zeros(B, cap, device=self.dev, dtype=torch.int32)
+            if K > 1:
+                st["cache"].kv_src = torch.zeros(B, cap, device=self.dev, dtype=torch.int32)
+                i32 = dict(device=self.dev, dtype=torch.int32)
+                st["beam"] = dict(
+                    lp=torch.empty(B, self.g.vocab_size, device=self.dev, dtype=F32),
+                    cand_val=torch.empty(B, _lib.BEAM_MAX_KEEP, device=self.dev, dtype=F32),
+                    cand_tok=torch.empty(B, _lib.BEAM_MAX_KEEP, **i32),
+                    running=torch.empty(B, device=self.dev, dtype=F32),
+                    fin_score=torch.empty(B, device=self.dev, dtype=F32),
+                    fin_info=torch.empty(B, 4, **i32), flags=torch.empty(B // K, 2, **i32),
+                    rec=torch.empty(cap, B, 2, **i32))
             self._gen_state = st
         return st
 
@@ -920,6 +994,117 @@ class U2Engine:
             outs = [torch.nn.functional.pad(o, (0, width - o.shape[1]), value=int(fill)) for o in outs]
         return torch.cat(outs, dim=0)
 
+    def _generate_beam(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id, use_graph: bool,
+                       beam: BeamSearch, lens: torch.Tensor, logits_out: Optional[list] = None) -> torch.Tensor:
+        """Beam search over B prompts: one prefill, the prompt KV replicated into the K beam rows of every prompt (as
+        _generate_multi does), then chunks of cap // K prompts per decode batch. Returns [B * num_return_sequences, n]
+        ids, best hypothesis first per prompt, cropped to the longest returned one and filled with HF's fill value.
+        logits_out (tests): receives every step's raw fp32 logits [rows, V] of each chunk, a list per chunk."""
+        K, n_ret = int(beam.num_beams), int(beam.num_return_sequences)
+        cap = 16 if self._use_tc_decode(16) else 8  # sequences one decode step can carry (dlinear N / gemv batch)
+        if K > cap:
+            raise ValueError(f"num_beams={K} exceeds the {cap} rows one decode step carries on this path")
+        if not 1 <= n_ret <= K:
+            raise ValueError(f"num_return_sequences={n_ret} must be in 1..num_beams={K}")
+        if eos_token_id is None:
+            eos = ()
+        elif isinstance(eos_token_id, torch.Tensor):
+            eos = tuple(int(e) for e in eos_token_id.reshape(-1).tolist())
+        else:
+            eos = tuple(int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id]))
+        if len(eos) > _lib.BEAM_MAX_EOS:
+            raise ValueError(f"beam search supports at most {_lib.BEAM_MAX_EOS} EOS ids, got {len(eos)}")
+        fill = (beam.pad_token_id or eos[0]) if eos else -1
+        B, L, _ = embeds.shape
+        pc = self.new_cache(B, L)
+        hidden = self.prefill(embeds, pc)
+        logits0 = self.lm_logits(self._last_hidden(hidden, lens))
+        per = cap // K
+        self._beam, self._beam_req = beam, (int(max_new_tokens), eos)
+        seqs, scores = [], []
+        try:
+            for p0 in range(0, B, per):
+                P = min(per, B - p0)
+                src_cpu = torch.arange(p0 * K, (p0 + P) * K) // K  # prompt of every beam row
+                src = src_cpu.to(self.dev)
+                st = self._gen_state_for(P * K, L + max_new_tokens)
+                cache = st["cache"]
+                cache.k[:, :, :, :L].copy_(pc.k.index_select(1, src))
+                cache.v[:, :, :, :L].copy_(pc.v.index_select(1, src))
+                cache.set_length(lens.index_select(0, src_cpu))
+                lo = None
+                if logits_out is not None:
+                    lo = []
+                    logits_out.append(lo)
+                self._beam_loop(st, logits0.index_select(0, src), max_new_tokens, use_graph, lo)
+                s, sc = self._beam_backtrack(st["beam"], P, K, n_ret, fill)
+                seqs += s
+                scores.append(sc)
+        finally:
+            self._beam = None
+        width = max(len(x) for x in seqs)
+        out = torch.full((len(seqs), width), fill, dtype=torch.int64)
+        for i, x in enumerate(seqs):
+            out[i, :len(x)] = torch.as_tensor(x, dtype=torch.int64)
+        self.last_beam_scores = torch.cat(scores)
+        return out.to(self.dev)
+
+    def _beam_loop(self, st, logits0: torch.Tensor, max_new_tokens: int, use_graph: bool, logits_out: Optional[list]):
+        """The first beam step on the prefill logits, then up to max_new_tokens - 1 decode steps (the steps after the
+        first replay one captured graph); every 16 steps the host checks whether every prompt is done."""
+        cache, bs = st["cache"], st["beam"]
+        R, K = cache.batch, self._beam.num_beams
+        bufs = self._decode_buffers(R)
+        self.reset_decode_state(R)
+        bs["running"].view(-1, K).fill_(-1e9)[:, 0] = 0.0
+        bs["fin_score"].fill_(-1e9)
+        bs["fin_info"].copy_(torch.tensor([0, -1, 0, 0], dtype=torch.int32).expand(R, 4))
+        bs["flags"].copy_(torch.tensor([1, 0], dtype=torch.int32).expand(R // K, 2))
+        cache.kv_src.copy_(torch.arange(R, device=self.dev, dtype=torch.int32)[:, None].expand(R, cache.max_len))
+        self._pick_next(logits0, bufs["ids"].view(R), None, step=0)
+        if logits_out is not None:
+            logits_out.append(logits0.float().clone())
+        graph, n_graph = st["graph"], st["n_graph"]
+        for step in range(1, max_new_tokens):
+            if step % 16 == 1 and bool(bs["flags"][:, 1].all()):
+                break
+            if use_graph and (graph is not None or step >= 2):
+                if graph is None:
+                    n0 = _lib.launches()
+                    graph = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(graph):
+                        self.decode_step(cache)
+                    n_graph = _lib.launches() - n0
+                    _lib.add_launches(-n_graph)  # capture records, it does not execute
+                    st["graph"], st["n_graph"] = graph, n_graph
+                graph.replay()
+                _lib.add_launches(n_graph)
+            else:
+                self.decode_step(cache)
+            if logits_out is not None:
+                logits_out.append(bufs["logits"].clone())
+
+    @staticmethod
+    def _beam_backtrack(bs: dict, P: int, K: int, n_ret: int, fill: int):
+        """The best n_ret finished hypotheses of every prompt, rebuilt from the per-step (token, parent beam) records."""
+        info = bs["fin_info"].cpu().numpy()
+        score = bs["fin_score"].cpu()
+        rec = bs["rec"].cpu().numpy()
+        seqs, keep = [], []
+        for p in range(P):
+            for i in range(n_ret):
+                r = p * K + i
+                _, te, beam, tok = (int(x) for x in info[r])
+                seq = [fill] * (te + 1)
+                if te >= 0:
+                    seq[te] = tok
+                    for s in range(te - 1, -1, -1):
+                        seq[s] = int(rec[s, p * K + beam, 0])
+                        beam = int(rec[s, p * K + beam, 1])
+                seqs.append(seq)
+                keep.append(r)
+        return seqs, score[keep]
+
     def _decode_loop(self, st, logits0: torch.Tensor, max_new_tokens: int, eos_token_id, use_graph: bool,
                      return_margins: bool, force_ids: Optional[torch.Tensor] = None, logits_out: Optional[list] = None):
         """Pick the first token from `logits0`, then run max_new_tokens - 1 decode steps on st['cache'] (whose length
@@ -998,6 +1183,7 @@ class KVCache:
         self.length = 0
         self.length_dev = torch.zeros(batch, device=device, dtype=torch.int32)
         self.length_plus1_dev = torch.ones(batch, device=device, dtype=torch.int32)
+        self.kv_src = None  # beam search: int32 [B, max_len], the cache row holding position t of sequence b
 
     def set_length(self, n):
         """n: one length for every sequence, or the per-sequence lengths [B]."""

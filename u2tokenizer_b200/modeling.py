@@ -495,9 +495,10 @@ class U2MetaForCausalLM(ABC):
                 inputs_embeds = eng.embed_tokens(inputs)
         else:
             inputs_embeds = eng.embed_tokens(inputs)
-        if kwargs.pop("num_beams", 1) != 1:
-            raise NotImplementedError("beam search is not implemented on the CUDA path (greedy and sampling are)")
         gc = getattr(self, "generation_config", None)
+        num_beams = kwargs.pop("num_beams", None)
+        if num_beams is None:
+            num_beams = getattr(gc, "num_beams", None) or 1
         do_sample = kwargs.pop("do_sample", None)
         if do_sample is None:
             do_sample = bool(getattr(gc, "do_sample", False))
@@ -524,13 +525,18 @@ class U2MetaForCausalLM(ABC):
         if pad is None and gc is not None:
             pad = gc.pad_token_id
         n_ret = int(opt("num_return_sequences", 1))
+        beam = None
+        if num_beams != 1:
+            beam = self._generate_beam_search(kwargs, gc, num_beams, bool(do_sample), n_ret, pad)
         procs = self._generate_logits_processors(kwargs, gc, L, eos, eng.g.vocab_size)
         self._check_remaining_generate_kwargs(kwargs)
-        if n_ret > 1 and not do_sample:
+        if n_ret > 1 and not do_sample and beam is None:
             raise ValueError("num_return_sequences > 1 needs do_sample=True (greedy decoding is deterministic; HF raises too)")
         ids = eng.generate(inputs_embeds.to(torch.bfloat16), max_new_tokens=max_new, eos_token_id=eos,
                            do_sample=bool(do_sample), temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
-                           num_return_sequences=n_ret, lengths=lengths, processors=procs)
+                           num_return_sequences=n_ret, lengths=lengths, processors=procs, beam=beam)
+        if beam is not None:
+            return ids  # HF's beam output: best hypotheses first, each filled after its end with pad or eos[0]
         if eos is not None:
             eos_t = torch.as_tensor(eos if isinstance(eos, (list, tuple)) else [eos], device=ids.device)
             hit = torch.isin(ids, eos_t)
@@ -541,6 +547,43 @@ class U2MetaForCausalLM(ABC):
             keep = int((~after).any(dim=0).sum())
             ids = ids[:, :max(keep, 1)]
         return ids  # new tokens only, like HF generate() on inputs_embeds (reference u2llama.py:123-127)
+
+    @staticmethod
+    def _generate_beam_search(kwargs: dict, generation_config, num_beams, do_sample: bool, num_return_sequences: int,
+                              pad_token_id):
+        """num_beams != 1: length_penalty and early_stopping (popped from `kwargs`, else read from `generation_config`)
+        -> a validated engine.BeamSearch. Beam sampling, group (diverse) and constrained beam search are refused."""
+        from .engine import BeamSearch
+
+        def opt(name, default):
+            v = kwargs.pop(name, None)
+            if v is None and generation_config is not None:
+                v = getattr(generation_config, name, None)
+            return default if v is None else v
+
+        if isinstance(num_beams, bool) or not isinstance(num_beams, (int, np.integer)) or num_beams < 1:
+            raise ValueError(f"`num_beams` has to be a positive integer, but is {num_beams!r}")
+        if do_sample:
+            raise NotImplementedError("beam sampling (num_beams > 1 with do_sample=True) is not implemented on the CUDA path")
+        if opt("num_beam_groups", 1) != 1:
+            raise NotImplementedError("group (diverse) beam search is not implemented on the CUDA path")
+        for k in ("constraints", "force_words_ids"):
+            if kwargs.pop(k, None):
+                raise NotImplementedError(f"constrained beam search ({k}) is not implemented on the CUDA path")
+        lp = opt("length_penalty", 1.0)
+        if isinstance(lp, bool) or not isinstance(lp, (int, float, np.integer, np.floating)) or not np.isfinite(lp):
+            raise ValueError(f"`length_penalty` has to be a finite number, but is {lp!r}")
+        es = opt("early_stopping", False)
+        if not (es is True or es is False or es == "never"):
+            raise ValueError(f"`early_stopping` has to be True, False or 'never', but is {es!r}")
+        if num_return_sequences > num_beams:
+            raise ValueError(f"`num_return_sequences` ({num_return_sequences}) has to be smaller or equal to "
+                             f"`num_beams` ({num_beams}).")
+        if pad_token_id is not None and not isinstance(pad_token_id, (int, np.integer)):
+            pad_token_id = int(torch.as_tensor(pad_token_id).reshape(-1)[0])
+        return BeamSearch(num_beams=int(num_beams), length_penalty=float(lp), early_stopping=es,
+                          num_return_sequences=int(num_return_sequences),
+                          pad_token_id=None if pad_token_id is None else int(pad_token_id))
 
     @staticmethod
     def _check_remaining_generate_kwargs(kwargs: dict):

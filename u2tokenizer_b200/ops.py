@@ -340,13 +340,23 @@ def rope(x: torch.Tensor, *, rows: int, ld: int, dh: int, n_q: int, n_k: int, n_
 
 def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, out: torch.Tensor, *,
                      B: int, Hq: int, Hkv: int, dh: int, Tmax: int, T: int = 0, T_dev=None, ldq: int, ldo: int,
-                     scale: float, T_per_seq: bool = False):
-    """T_per_seq: sequence b attends over T_dev[b] keys (int32 [B])."""
-    _need_cuda(q, k_cache, v_cache, out, T_dev)
+                     scale: float, T_per_seq: bool = False, kv_src: Optional[torch.Tensor] = None):
+    """T_per_seq: sequence b attends over T_dev[b] keys (int32 [B]).
+    kv_src (beam search): int32 [B, >= Tmax]; key t of sequence b is read from cache row kv_src[b, t]."""
+    _need_cuda(q, k_cache, v_cache, out, T_dev, kv_src)
+    _check_kv_src(kv_src, B, Tmax)
     _lib.check(_lib.load().u2_decode_attention_bf16(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                                     out.data_ptr(), B, Hq, Hkv, dh, Tmax, T, _ptr(T_dev), ldq, ldo,
-                                                    scale, 1 if T_per_seq else 0, _stream()), "u2_decode_attention_bf16")
+                                                    scale, 1 if T_per_seq else 0, _ptr(kv_src),
+                                                    kv_src.stride(0) if kv_src is not None else 0, _stream()),
+               "u2_decode_attention_bf16")
     return out
+
+
+def _check_kv_src(kv_src: Optional[torch.Tensor], B: int, Tmax: int) -> None:
+    if kv_src is not None and (kv_src.dtype != torch.int32 or kv_src.dim() != 2 or kv_src.shape[0] != B
+                               or kv_src.shape[1] < Tmax or kv_src.stride(1) != 1):
+        raise ValueError(f"kv_src must be int32 [{B}, >= {Tmax}] with unit column stride")
 
 
 def gemv(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, residual=None, norm_gamma=None,
@@ -466,11 +476,14 @@ def decode_embed(ids: torch.Tensor, table: torch.Tensor, gamma: torch.Tensor, x:
 def decode_attention_fused(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, out: torch.Tensor, *,
                            B: int, Hq: int, Hkv: int, dh: int, Tmax: int, inv_freq: torch.Tensor, scale: float,
                            pos: int = 0, pos_dev=None, q_norm_w=None, k_norm_w=None, eps: float = 1e-6, kv_splits: int = 1,
-                           pdl: bool = False, pos_per_seq: bool = False):
+                           pdl: bool = False, pos_per_seq: bool = False, kv_src: Optional[torch.Tensor] = None):
     """q/k norm + RoPE + KV-cache append + GQA attention for one new token per sequence (one launch).
     kv_splits in {2, 4, 8}: a cluster of that many CTAs per (sequence, KV head) splits the cached keys.
-    pos_per_seq: sequence b's new token sits at position pos_dev[b] (int32 [B]) instead of pos_dev[0]."""
-    _need_cuda(qkv, k_cache, v_cache, out, inv_freq, pos_dev, q_norm_w, k_norm_w)
+    pos_per_seq: sequence b's new token sits at position pos_dev[b] (int32 [B]) instead of pos_dev[0].
+    kv_src (beam search): int32 [B, >= Tmax]; the cached key / value t < pos of sequence b is read from cache row
+    kv_src[b, t] (the new token is appended to and read from row b). None: every sequence reads its own row."""
+    _need_cuda(qkv, k_cache, v_cache, out, inv_freq, pos_dev, q_norm_w, k_norm_w, kv_src)
+    _check_kv_src(kv_src, B, Tmax)
     d = _lib.FusedDecodeDesc()
     d.B, d.Hq, d.Hkv, d.dh, d.Tmax, d.pos = B, Hq, Hkv, dh, Tmax, pos
     d.pos_dev = _ptr(pos_dev)
@@ -481,6 +494,8 @@ def decode_attention_fused(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: to
     d.kv_splits = int(kv_splits)
     d.pdl = 1 if pdl else 0
     d.pos_per_seq = 1 if pos_per_seq else 0
+    d.kv_src = _ptr(kv_src)
+    d.ld_kv_src = kv_src.stride(0) if kv_src is not None else 0
     _lib.check(_lib.load().u2_decode_attention_fused_bf16(qkv.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                                           out.data_ptr(), C.byref(d), _stream()),
                "u2_decode_attention_fused_bf16")
@@ -634,6 +649,88 @@ def logits_process(logits: torch.Tensor, params: torch.Tensor, ids: torch.Tensor
                                                  hist.data_ptr(), hist.stride(0), hist.shape[1], params.data_ptr(),
                                                  _ptr(step_dev), int(step), _stream()), "u2_logits_process_f32")
     return logits
+
+
+def log_softmax(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Row-wise log_softmax of fp32 [rows, V] into `out` (a separate fp32 buffer)."""
+    _need_cuda(x, out)
+    if x.dtype != F32 or x.dim() != 2 or x.stride(1) != 1:
+        raise TypeError("log_softmax expects fp32 rows with unit column stride")
+    if out is None:
+        out = torch.empty_like(x)
+    if out.dtype != F32 or out.shape != x.shape or out.stride(1) != 1:
+        raise ValueError("log_softmax: out must be fp32 shaped like x")
+    _lib.check(_lib.load().u2_log_softmax_f32(x.data_ptr(), out.data_ptr(), x.shape[0], x.shape[1], x.stride(0),
+                                              out.stride(0), _stream()), "u2_log_softmax_f32")
+    return out
+
+
+EARLY_STOPPING = {False: 0, True: 1, "never": 2}
+
+
+def beam_params(device, *, num_beams: int, length_penalty: float = 1.0, early_stopping=False, max_new_tokens: int,
+                eos_token_ids=(), out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The u2_beam_params block (include/u2b200.h) in device memory, as uint8. `out` (a block made earlier) is overwritten
+    in place, so a captured decode graph gets a new request's values without a new capture. beams_to_keep is HF's
+    max(2, 1 + n_eos) * num_beams."""
+    K, eos = int(num_beams), [int(e) for e in eos_token_ids]
+    if not 2 <= K <= _lib.BEAM_MAX_BEAMS:
+        raise ValueError(f"num_beams must be in 2..{_lib.BEAM_MAX_BEAMS}, got {num_beams}")
+    if len(eos) > _lib.BEAM_MAX_EOS:
+        raise ValueError(f"beam search supports at most {_lib.BEAM_MAX_EOS} EOS ids, got {len(eos)}")
+    if not (early_stopping is True or early_stopping is False or early_stopping == "never"):
+        raise ValueError(f"early_stopping must be True, False or 'never', got {early_stopping!r}")
+    if int(max_new_tokens) < 1:
+        raise ValueError("max_new_tokens must be >= 1")
+    blk = _lib.BeamParams()
+    blk.length_penalty = float(length_penalty)
+    blk.num_beams, blk.beams_to_keep = K, max(2, 1 + len(eos)) * K
+    blk.early_stopping, blk.max_new_tokens, blk.n_eos = EARLY_STOPPING[early_stopping], int(max_new_tokens), len(eos)
+    for i, e in enumerate(eos):
+        blk.eos[i] = e
+    host = torch.frombuffer(bytearray(bytes(blk)), dtype=torch.uint8)
+    if out is None:
+        return host.to(device)
+    out.copy_(host)
+    return out
+
+
+def beam_topk(logprobs: torch.Tensor, running: torch.Tensor, flags: torch.Tensor, params: torch.Tensor,
+              cand_val: torch.Tensor, cand_tok: torch.Tensor):
+    """Per row, the top beams_to_keep of logprobs[r] + running[r] into cand_val / cand_tok [rows, BEAM_MAX_KEEP]."""
+    _need_cuda(logprobs, running, flags, params, cand_val, cand_tok)
+    R, V = logprobs.shape
+    if logprobs.dtype != F32 or logprobs.stride(1) != 1:
+        raise TypeError("beam_topk: fp32 log-probs with unit column stride")
+    if cand_val.shape != (R, _lib.BEAM_MAX_KEEP) or cand_tok.shape != (R, _lib.BEAM_MAX_KEEP):
+        raise ValueError(f"beam_topk: candidates must be [{R}, {_lib.BEAM_MAX_KEEP}]")
+    _lib.check(_lib.load().u2_beam_topk_f32(logprobs.data_ptr(), logprobs.stride(0), R, V, running.data_ptr(),
+                                            flags.data_ptr(), params.data_ptr(), cand_val.data_ptr(),
+                                            cand_tok.data_ptr(), _stream()), "u2_beam_topk_f32")
+
+
+def beam_step(params: torch.Tensor, st: dict, ids: torch.Tensor, kv_src: torch.Tensor, pos_dev: torch.Tensor, *,
+              V: int, hist: Optional[torch.Tensor] = None, step: int = 0, step_dev=None):
+    """One CTA per prompt: merge the row candidates, update the beam state `st` (tensors 'cand_val', 'cand_tok',
+    'running', 'fin_score', 'fin_info', 'flags', 'rec'; see u2_beam_step_desc) and write the next ids [rows] int64,
+    the reordered kv_src and (optional) processor history."""
+    d = _lib.BeamStepDesc()
+    d.params = params.data_ptr()
+    d.prompts, d.V = st["flags"].shape[0], int(V)
+    for k in ("cand_val", "cand_tok", "running", "fin_score", "fin_info", "flags"):
+        _need_cuda(st[k])
+        setattr(d, k, st[k].data_ptr())
+    _need_cuda(ids, kv_src, pos_dev, hist, step_dev)
+    if ids.dtype != torch.int64 or kv_src.dtype != torch.int32 or not kv_src.is_contiguous():
+        raise ValueError("beam_step: ids int64, kv_src contiguous int32")
+    d.ids = ids.data_ptr()
+    d.rec, d.ld_rec, d.rec_rows = st["rec"].data_ptr(), st["rec"].stride(0), st["rec"].shape[0]
+    d.kv_src, d.ld_kv_src = kv_src.data_ptr(), kv_src.stride(0)
+    d.pos_dev = pos_dev.data_ptr()
+    if hist is not None:
+        d.hist, d.ld_hist, d.hist_cap = hist.data_ptr(), hist.stride(0), hist.shape[1]
+    d.step_dev = _ptr(step_dev)
+    _lib.check(_lib.load().u2_beam_step(C.byref(d), int(step), _stream()), "u2_beam_step")
 
 
 def lmhead_logprob(hidden: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor, *, want_lse: bool = False,
