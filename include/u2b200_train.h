@@ -167,6 +167,37 @@ U2_API int u2_add_bf16(void* dst, const void* src, int64_t n, void* stream);
 U2_API int u2_cast_f32_bf16(const float* in, void* out, int64_t n, void* stream);
 U2_API int u2_cast_bf16_f32(const void* in, float* out, int64_t n, void* stream);
 
+/* LoRA adapters of the decoder linears (PEFT LoraLayer.forward: y = W x + s * B_j A_j dropout_j(x), s = lora_alpha / r;
+ * reference src/train/train_stage1.py:342-353). The 1-3 adapters of one call share the input X [M, K] (q|k|v, gate|up,
+ * or o / down alone); their A matrices are stacked [n_adapters * r, K] (row stride K), U / dU are [M, n_adapters * r]
+ * with adapter j in columns [j r, (j + 1) r). r in {8, 16, 32, 64}; bf16 data, fp32 accumulation.
+ *
+ * Dropout mask (inverted dropout, one independent mask per adapter as PEFT has one nn.Dropout per LoRA layer):
+ *   fmix32(h) = h ^= h >> 16; h *= 0x85EBCA6B; h ^= h >> 13; h *= 0xC2B2AE35; h ^= h >> 16      (uint32 arithmetic)
+ *   key_j     = fmix32(lo32(seed) ^ fmix32(hi32(seed) + stream[j] * 0x9E3779B9))
+ *   h         = fmix32(fmix32(key_j ^ row) ^ col)                  (row of X in [0, M), column in [0, K))
+ *   D_j(row, col) = 0 if h < floor(p * 2^32), else 1 / (1 - p)     (p = 0: every element kept, D = 1)
+ * stream[j] names the adapter: the training engine passes layer * 8 + t with t = 0..6 for q, k, v, o, gate, up, down.
+ * The masked input D_j o X is rounded to bf16 (the dtype PEFT's dropout returns) wherever it is an operand.
+ *
+ *   u2_lora_down_bf16:  U[:, j] = s * (D_j o X) A_j^T
+ *   u2_lora_wgrad_bf16: dA_j = s * dU_j^T (D_j o X)      written to the stacked bf16 gradient [n_adapters * r, K]
+ *                       (accumulate != 0: added to what it holds)
+ *   u2_lora_dgrad_bf16: dX += sum_j D_j o (s * dU_j A_j) (in place, row stride ldx)
+ * ldx is the row stride of X (down, wgrad) or dX (dgrad); ldu that of U / dU. */
+typedef struct u2_lora_desc {
+  int32_t M, K, r, n_adapters;
+  int64_t ldx, ldu;
+  float scale;
+  float p;
+  uint64_t seed;
+  int32_t stream[3];
+  int32_t accumulate;
+} u2_lora_desc;
+U2_API int u2_lora_down_bf16(const void* X, const void* A, void* U, const u2_lora_desc* desc, void* stream);
+U2_API int u2_lora_wgrad_bf16(const void* dU, const void* X, void* dA, const u2_lora_desc* desc, void* stream);
+U2_API int u2_lora_dgrad_bf16(const void* dU, const void* A, void* dX, const u2_lora_desc* desc, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -191,6 +191,18 @@ class AdamWDesc(C.Structure):
     ]
 
 
+class LoraDesc(C.Structure):
+    """Mirror of ``u2_lora_desc`` (include/u2b200_train.h)."""
+    _fields_ = [
+        ("M", C.c_int32), ("K", C.c_int32), ("r", C.c_int32), ("n_adapters", C.c_int32),
+        ("ldx", C.c_int64), ("ldu", C.c_int64),
+        ("scale", C.c_float), ("p", C.c_float),
+        ("seed", C.c_uint64),
+        ("stream", C.c_int32 * 3),
+        ("accumulate", C.c_int32),
+    ]
+
+
 LP_MAX_EOS, LP_MAX_BAD_WORDS, LP_MAX_BAD_TOKENS = 8, 256, 2048  # U2_LP_MAX_* of include/u2b200.h
 
 
@@ -304,6 +316,9 @@ SIGNATURES = {
     "u2_add_bf16": (C.c_int, [_P, _P, _L, _P]),
     "u2_cast_f32_bf16": (C.c_int, [_P, _P, _L, _P]),
     "u2_cast_bf16_f32": (C.c_int, [_P, _P, _L, _P]),
+    "u2_lora_down_bf16": (C.c_int, [_P, _P, _P, C.POINTER(LoraDesc), _P]),
+    "u2_lora_wgrad_bf16": (C.c_int, [_P, _P, _P, C.POINTER(LoraDesc), _P]),
+    "u2_lora_dgrad_bf16": (C.c_int, [_P, _P, _P, C.POINTER(LoraDesc), _P]),
 }
 
 

@@ -191,7 +191,11 @@ class U2MetaForCausalLM(ABC):
             if not p.is_cuda:
                 raise RuntimeError("the mu2 hot path runs on CUDA only: move the model to an H100 (model.cuda()); "
                                    "there is no CPU fallback")
-            sd = {k: v for k, v in self.state_dict().items()}
+            if self.__dict__.get("_u2_lora") is not None:
+                from .lora import merged_state_dict
+                sd = merged_state_dict(self)   # LoRA: the decode step runs on W + s B A, no per-token adapter work
+            else:
+                sd = {k: v for k, v in self.state_dict().items()}
             eng = U2Engine(Geometry.from_hf(self.config), sd, device=p.device)
             self.__dict__["_u2_engine"] = eng
             self.__dict__["_u2_engine_stamp"] = self._param_stamp()
@@ -225,14 +229,16 @@ class U2MetaForCausalLM(ABC):
             if not p.is_cuda:
                 raise RuntimeError("the training path runs on CUDA only (model.cuda()); there is no CPU fallback")
 
-            def any_rg(prefix):
-                ps = [q for n, q in self.named_parameters() if n.startswith(prefix)]
+            def any_rg(prefix):   # LoRA adapters always train: they do not make their group trainable
+                ps = [q for n, q in self.named_parameters() if n.startswith(prefix) and ".lora_" not in n]
                 return any(q.requires_grad for q in ps) if ps else False
             flags = dict(vit=any_rg("model.vision_tower."), proj=any_rg("model.mm_projector."), u2t=any_rg("model.u2tokenizer."),
                          dec=any_rg("model.layers.") or any_rg("model.norm."), embed=any_rg("model.embed_tokens."),
                          head=any_rg("lm_head."))
             kw.setdefault("trainable", flags)
-            te = TrainEngine(Geometry.from_hf(self.config), self.state_dict(), device=p.device, **kw)
+            lora = self.__dict__.get("_u2_lora")
+            sd = {k.replace(".base_layer.", "."): v for k, v in self.state_dict().items()}
+            te = TrainEngine(Geometry.from_hf(self.config), sd, device=p.device, lora=lora, **kw)
             te.bind_module(self)
             self.__dict__["_u2_train_engine"] = te
             self.invalidate_engine()

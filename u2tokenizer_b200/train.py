@@ -19,6 +19,7 @@ No arithmetic in torch: torch provides memory, streams, NCCL. There is no CPU pa
 from __future__ import annotations
 
 import math
+from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -31,6 +32,27 @@ from .synthetic import param_shapes
 
 BF16, F32 = torch.bfloat16, torch.float32
 _VEC_SUFFIX = ("relative_bias", "dynamic_pool.gate_fc.weight", "cls_token", "position_embeddings", "query_tokens")
+
+
+# LoRA targets of one decoder layer in mask-stream order (u2_lora_desc.stream = layer * 8 + index), grouped as the training
+# forward runs them: the members of a group share one input and one fused base GEMM
+LORA_TARGETS = ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj")
+LORA_GROUPS = (("self_attn.", ("q_proj", "k_proj", "v_proj")), ("self_attn.", ("o_proj",)), ("mlp.", ("gate_proj", "up_proj")),
+               ("mlp.", ("down_proj",)))
+
+
+@dataclass(frozen=True)
+class LoraSpec:
+    """LoRA adapters on the decoder linears: rank r, scaling = lora_alpha / r, dropout p, short names of the targets."""
+    r: int
+    scaling: float
+    dropout: float
+    targets: Tuple[str, ...]
+
+    def names(self, layer: int, prefix: str, t: str) -> Tuple[str, str, str]:
+        """(base weight, lora_A, lora_B) parameter names of target t of a layer (PEFT's module layout)."""
+        m = f"model.layers.{layer}.{prefix}{t}."
+        return m + "weight", m + "lora_A.default.weight", m + "lora_B.default.weight"
 
 
 def is_vector_param(name: str, shape) -> bool:
@@ -51,12 +73,17 @@ def training_order(g: Geometry) -> Tuple[List[str], List[str]]:
 
 
 class Layout:
-    """Offsets of every parameter in the flat buffers. W (bf16): [matrix region | vector region]; Gm (bf16): matrix
-    region; V32 / Gv (fp32): vector region."""
+    """Offsets of every parameter in the flat buffers. W (bf16): [matrix region | vector region | frozen region]; Gm
+    (bf16): matrix region; V32 / Gv (fp32): vector region. The frozen region holds the base weights of the LoRA targets
+    (empty without LoRA): no gradient slot, no optimizer state. With LoRA the matrix region holds the adapters in place
+    of those base weights, the A's of a fused group adjacent (q|k|v, gate|up), then its B's."""
 
-    def __init__(self, g: Geometry, world_size: int = 1, bucket_elems: int = 200_000_000):
-        self.shapes = param_shapes(g)
+    def __init__(self, g: Geometry, world_size: int = 1, bucket_elems: int = 200_000_000, lora: Optional[LoraSpec] = None):
+        self.shapes = dict(param_shapes(g))
         mats, vecs = training_order(g)
+        self.frozen_names: List[str] = []
+        if lora is not None:
+            mats = self._lora_order(g, mats, lora)
         self.mat_names, self.vec_names = mats, vecs
         self.mat_off, self.vec_off = {}, {}
         off = 0
@@ -85,6 +112,36 @@ class Layout:
             self.vec_off[n] = off
             off += (self._numel(n) + 7) // 8 * 8
         self.vec_total = max(8, off)
+        self.frozen_off = {}
+        off = 0
+        for n in self.frozen_names:
+            self.frozen_off[n] = off
+            off += (self._numel(n) + 7) // 8 * 8
+        self.frozen_total = off
+
+    def _lora_order(self, g: Geometry, mats: List[str], lora: LoraSpec) -> List[str]:
+        """The matrix order with every target's base weight replaced by its adapters (the base moves to frozen_names)."""
+        first = {}   # base name of a group's first targeted member -> the group's adapter names (A's, then B's)
+        skip = set()
+        for li in range(g.num_hidden_layers):
+            for pre, members in LORA_GROUPS:
+                tg = [t for t in members if t in lora.targets]
+                if not tg:
+                    continue
+                trip = [lora.names(li, pre, t) for t in tg]
+                for base, a, b in trip:
+                    out_f, in_f = self.shapes[base]
+                    self.shapes[a], self.shapes[b] = (lora.r, in_f), (out_f, lora.r)
+                    skip.add(base)
+                first[trip[0][0]] = [a for _, a, _ in trip] + [b for _, _, b in trip]
+        out = []
+        for n in mats:
+            if n in skip:
+                self.frozen_names.append(n)
+                out.extend(first.get(n, ()))
+            else:
+                out.append(n)
+        return out
 
     def _numel(self, n: str) -> int:
         k = 1
@@ -93,7 +150,7 @@ class Layout:
         return k
 
     def adjacent(self, names: Sequence[str]) -> bool:
-        tab = self.mat_off if names[0] in self.mat_off else self.vec_off
+        tab = next(t for t in (self.mat_off, self.vec_off, self.frozen_off) if names[0] in t)
         for a, b in zip(names[:-1], names[1:]):
             if tab[a] + self._numel(a) != tab[b]:
                 return False
@@ -110,7 +167,8 @@ class Var:
 
 class TrainEngine:
     def __init__(self, geom: Geometry, state_dict: Dict[str, torch.Tensor], device="cuda", world_size: int = 1, rank: int = 0,
-                 group=None, trainable: Optional[Dict[str, bool]] = None, bucket_elems: int = 200_000_000):
+                 group=None, trainable: Optional[Dict[str, bool]] = None, bucket_elems: int = 200_000_000,
+                 lora: Optional[LoraSpec] = None):
         if not torch.cuda.is_available():
             raise RuntimeError("TrainEngine needs a CUDA device: the training path has no CPU implementation")
         from . import _lib
@@ -121,16 +179,22 @@ class TrainEngine:
         self.dev = torch.device(device)
         self.world, self.rank, self.group = world_size, rank, group
         self.bucket_elems = bucket_elems
-        self.lay = Layout(g, world_size=world_size, bucket_elems=bucket_elems)
+        if lora is not None:
+            bad = [t for t in lora.targets if t not in LORA_TARGETS]
+            if bad or lora.r not in (8, 16, 32, 64) or not 0.0 <= lora.dropout < 1.0:
+                raise NotImplementedError(f"LoRA on the training path: targets in {LORA_TARGETS}, r in (8, 16, 32, 64), "
+                                          f"0 <= dropout < 1 (got {lora})")
+        self.lora = lora
+        self.lay = Layout(g, world_size=world_size, bucket_elems=bucket_elems, lora=lora)
         L = self.lay
-        self.W = torch.zeros(L.mat_total + L.vec_total, device=self.dev, dtype=BF16)
+        self.W = torch.zeros(L.mat_total + L.vec_total + L.frozen_total, device=self.dev, dtype=BF16)
         self.V32 = torch.zeros(L.vec_total, device=self.dev, dtype=F32)
         self.Gm = torch.zeros(L.mat_total, device=self.dev, dtype=BF16)
         self.Gv = torch.zeros(L.vec_total, device=self.dev, dtype=F32)
-        for n in L.mat_names + L.vec_names:
+        for n in L.mat_names + L.vec_names + L.frozen_names:
             if n in state_dict:
                 self.w(n).copy_(state_dict[n].to(self.dev).view(L.shapes[n]))
-            elif n == "lm_head.weight":
+            elif n == "lm_head.weight" or ".lora_" in n:
                 raise KeyError(n)
         self.tied = g.tie_word_embeddings or "lm_head.weight" not in L.shapes
         self.refresh_vectors()
@@ -160,6 +224,7 @@ class TrainEngine:
         self._gm_dirty = set()
         self._gm_offs = sorted((L.mat_off[n], n) for n in L.mat_names)
         self._gm_names_cache = {}
+        self._lora_seed = 0   # dropout-mask seed of the current forward (0 with p = 0 or outside a training forward)
 
     # =========================================================================================
     # flat-buffer views
@@ -168,6 +233,8 @@ class TrainEngine:
         L = self.lay
         if n in L.mat_off:
             return L.mat_off[n], L._numel(n), True
+        if n in L.frozen_off:
+            return L.mat_total + L.vec_total + L.frozen_off[n], L._numel(n), False
         return L.mat_total + L.vec_off[n], L._numel(n), False
 
     def w(self, n: str) -> torch.Tensor:
@@ -181,7 +248,7 @@ class TrainEngine:
         assert L.adjacent(names), names
         cols = L.shapes[names[0]][-1]
         k = sum(L._numel(n) for n in names)
-        off = L.mat_off[names[0]]
+        off = self._slot(names[0])[0]
         return self.W[off:off + k].view(k // cols, cols)
 
     def v32(self, n: str) -> torch.Tensor:
@@ -217,13 +284,14 @@ class TrainEngine:
     def refresh_vectors(self):
         """fp32 mirrors of the vector parameters (biases, norm weights, bias tables) from their bf16 values."""
         L = self.lay
-        T.cast(self.W[L.mat_total:], self.V32)
+        T.cast(self.W[L.mat_total:L.mat_total + L.vec_total], self.V32)
 
     def bind_module(self, model) -> None:
         """Re-point the module's nn.Parameters at the flat buffer (no second copy of the weights); gradients are
         exposed the same way after backward (see grads_for_module)."""
         sd_names = dict(model.named_parameters())
         for n, p in sd_names.items():
+            n = n.replace(".base_layer.", ".")   # a LoRA target's base weight (PEFT module layout)
             if n in self.lay.shapes:
                 p.data = self.w(n)
         if self.tied and "lm_head.weight" in sd_names:
@@ -942,8 +1010,7 @@ class TrainEngine:
             l = f"model.layers.{li}."
             self._mark([k for k in self.lay.mat_names if k.startswith(l)])
             y = self.rmsnorm(x, l + "input_layernorm.weight", "dec", eps)
-            wn = [l + "self_attn.q_proj.weight", l + "self_attn.k_proj.weight", l + "self_attn.v_proj.weight"]
-            qkv_raw = self.linear(y, self.wcat(wn), self.gm(wn) if tr else None)
+            qkv_raw = self._dec_linear(y, li, 0, tr)
             qkv = self._rope_dec(qkv_raw, l, B, Lx)
             qv = lambda t: t.view(B, Lx, nh, dh)[:, :, :hq]
             kv_ = lambda t: t.view(B, Lx, nh, dh)[:, :, hq:hq + hkv]
@@ -951,14 +1018,70 @@ class TrainEngine:
             ctx = self.attention(qkv, qv, qkv, kv_, qkv, vv_, (B, Lx, hq * dh), 1.0 / math.sqrt(dh), causal=True, group="dec")
             c2 = Var(ctx.v.view(B * Lx, hq * dh), ctx.ng)
             self._alias(c2, ctx)
-            x = self.linear(c2, self.w(l + "self_attn.o_proj.weight"), self.gm(l + "self_attn.o_proj.weight") if tr else None,
-                            residual=x)
+            x = self._dec_linear(c2, li, 1, tr, residual=x)
             y = self.rmsnorm(x, l + "post_attention_layernorm.weight", "dec", eps)
-            wg = [l + "mlp.gate_proj.weight", l + "mlp.up_proj.weight"]
-            gu = self.linear(y, self.wcat(wg), self.gm(wg) if tr else None)
+            gu = self._dec_linear(y, li, 2, tr)
             act = self.silu_mul(gu)
-            x = self.linear(act, self.w(l + "mlp.down_proj.weight"), self.gm(l + "mlp.down_proj.weight") if tr else None, residual=x)
+            x = self._dec_linear(act, li, 3, tr, residual=x)
         return self.rmsnorm(x, "model.norm.weight", "dec", eps)
+
+    def _dec_linear(self, x: Var, li: int, gi: int, tr: bool, residual: Optional[Var] = None) -> Var:
+        """Fused group gi of LORA_GROUPS of decoder layer li (q|k|v, o, gate|up, down). Without adapters: one linear
+        (wgrad when `tr`). With adapters on (some of) its members: the base output on the frozen weight, then for every
+        adapter j  U_j = s (D_j o x) A_j^T (lora_down) and y[:, rows_j] += U_j B_j^T on the GEMM (K = r)."""
+        pre, members = LORA_GROUPS[gi]
+        names = [f"model.layers.{li}.{pre}{t}.weight" for t in members]
+        lo = self.lora
+        tg = [t for t in members if lo is not None and t in lo.targets]
+        if not tg:
+            return self.linear(x, self.wcat(names), self.gm(names) if tr else None, residual=residual)
+        if len(tg) != len(members):
+            raise NotImplementedError(f"LoRA on part of a fused group ({tg} of {members}) is not supported on the training path")
+        r, s = lo.r, lo.scaling
+        trip = [lo.names(li, pre, t) for t in tg]
+        an, bn = [a for _, a, _ in trip], [b for _, _, b in trip]
+        A, Wb = self.wcat(an), self.wcat(names)
+        Bs = [self.w(b) for b in bn]
+        streams = [li * 8 + LORA_TARGETS.index(t) for t in tg]
+        p, seed = (lo.dropout, self._lora_seed) if self._lora_seed else (0.0, 0)
+        y = ops.linear(x.v, Wb, residual=residual.v if residual is not None else None)
+        x2 = x.v.view(-1, x.v.shape[-1])
+        U = T.lora_down(x2, A, r, s, p=p, seed=seed, streams=streams)
+        y2 = y.view(-1, y.shape[-1])
+        M, Ntot = y2.shape
+        col = 0
+        cols = []
+        for j, B in enumerate(Bs):
+            n = B.shape[0]
+            yj, uj = y2[:, col:col + n], U[:, j * r:(j + 1) * r]
+            ops.gemm(uj, B, yj, M=M, N=n, K=r, lda=U.stride(0), ldb=r, ldc=Ntot, residual=yj, ldr=Ntot)
+            cols.append((col, n))
+            col += n
+        out = Var(y, True)
+
+        def bwd():
+            dy = out.g
+            if dy is None:
+                return
+            dy2 = dy.view(-1, Ntot)
+            dU = torch.empty_like(U)
+            for j, (c0, n) in enumerate(cols):
+                dyj = dy2[:, c0:c0 + n]
+                self.wgrad(dyj, U[:, j * r:(j + 1) * r], self.gm(bn[j]))
+                T.linear_dgrad(dyj, Bs[j], out=dU[:, j * r:(j + 1) * r])
+            gA = self.gm(an)
+            T.lora_wgrad(dU, x2, gA, r, s, p=p, seed=seed, streams=streams, accumulate=self._gm_begin_write(gA))
+            if x.ng:
+                if x.g is None:
+                    x.g = T.linear_dgrad(dy, Wb)
+                else:
+                    T.linear_dgrad(dy, Wb, out=x.g, accumulate=True)
+                T.lora_dgrad(dU, A, x.g.view(-1, x2.shape[1]), r, s, p=p, seed=seed, streams=streams)
+            if residual is not None:
+                self._acc(residual, dy, owned=True)
+            out.g = None
+        self.tape.append(bwd)
+        return out
 
     def _rope_dec(self, qkv_raw: Var, l: str, B: int, Lx: int) -> Var:
         g = self.g
@@ -1057,11 +1180,19 @@ class TrainEngine:
         self._pending = None
         self._gm_clear_stale(tuple(self._gm_dirty))   # whatever no marker covered
 
+    def _draw_lora_seed(self):
+        """LoRA dropout of a training forward: one nonzero 63-bit seed from torch's default generator (torch.manual_seed
+        makes the masks reproducible); the tape keeps it and the backward recomputes the masks from it."""
+        self._lora_seed = 0
+        if self.lora is not None and self.lora.dropout > 0:
+            self._lora_seed = int(torch.randint(1, 2 ** 63 - 1, (1,)).item())
+
     def forward_loss(self, images, input_ids, question_ids, labels) -> torch.Tensor:
         """Forward half of the training step: HF ForCausalLMLoss of `model(images=, input_ids=, question_ids=, labels=)`
         (reference u2llama.py:76-87: shift by one, mean NLL over labels != -100). Keeps the tape for backward()."""
         self.tape = []
         self.refresh_vectors()
+        self._draw_lora_seed()
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         lab = labels.to(self.dev, torch.int64)
         shift = torch.full_like(lab, -100)
@@ -1090,6 +1221,7 @@ class TrainEngine:
     def forward_loss_only(self, images, input_ids, question_ids, labels) -> torch.Tensor:
         self.tape = []
         self.refresh_vectors()
+        self._lora_seed = 0
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         lab = labels.to(self.dev, torch.int64)
         shift = torch.full_like(lab, -1)
@@ -1105,6 +1237,7 @@ class TrainEngine:
         DPO step, trl DPOTrainer.compute_ref_log_probs / dpo_u2trainer.py:267-302)."""
         self.tape = []
         self.refresh_vectors()
+        self._lora_seed = 0
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         labels, mask = _dpo_labels(input_ids.to(self.dev), loss_mask.to(self.dev))
         hname, Wh = self._head_w()
@@ -1118,6 +1251,7 @@ class TrainEngine:
         reference model. Returns the fp32 [3] stats tensor (loss, reward accuracy, reward margin)."""
         self.tape = []
         self.refresh_vectors()
+        self._draw_lora_seed()
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         labels, mask = _dpo_labels(input_ids.to(self.dev), loss_mask.to(self.dev))
         stats = {}
@@ -1148,7 +1282,7 @@ class TrainEngine:
             lo = i * L.bucket + self.rank * pc
             T.cast(self.W[lo:lo + pc], mm[i * pc:(i + 1) * pc])
         vm = torch.empty(L.vec_total, device=self.dev, dtype=F32)
-        T.cast(self.W[L.mat_total:], vm)
+        T.cast(self.W[L.mat_total:L.mat_total + L.vec_total], vm)
         self.opt = dict(lr=lr, b1=betas[0], b2=betas[1], eps=eps, wd=weight_decay, clip=max_grad_norm, step=0,
                         m_master=mm, m_m=torch.zeros(nb * pc, device=self.dev, dtype=moment_dtype),
                         m_v=torch.zeros(nb * pc, device=self.dev, dtype=moment_dtype),
@@ -1221,7 +1355,8 @@ class TrainEngine:
                     done = torch.cuda.Event()
                     done.record(self.comm_stream)
                 self._ag_ev[i] = done
-        T.adamw(o["v_master"], o["v_m"], o["v_v"], self.Gv, self.W[L.mat_total:], param_out_f32=self.V32, **kw)
+        T.adamw(o["v_master"], o["v_m"], o["v_v"], self.Gv, self.W[L.mat_total:L.mat_total + L.vec_total], param_out_f32=self.V32,
+                **kw)
         o["reduced"] = [False] * nb
 
     def grads_for_module(self, model) -> None:

@@ -332,3 +332,64 @@ def linear_wgrad(dy: torch.Tensor, x: torch.Tensor, out: torch.Tensor, *, accumu
     ops.gemm(dy2, x2, out, M=N, N=K, K=M, lda=dy2.stride(0), ldb=x2.stride(0), ldc=out.stride(0), a_mn=True, b_mn=True,
              residual=out if accumulate else None, ldr=out.stride(0) if accumulate else 0)
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# LoRA adapters (csrc/lora.cu): the masked down-projection and its two masked gradients
+# ------------------------------------------------------------------------------------------------
+def _lora_desc(x2: torch.Tensor, u2: torch.Tensor, A: torch.Tensor, r: int, scale: float, p: float, seed: int, streams,
+               accumulate: bool = False):
+    M, K = x2.shape
+    nA = A.shape[0] // r
+    if A.shape != (nA * r, K) or not A.is_contiguous() or not 1 <= nA <= 3:
+        raise ValueError(f"lora: A must be the contiguous stack [n_adapters * r, K] of 1-3 adapters, got {tuple(A.shape)}")
+    if u2.shape != (M, nA * r) or u2.stride(1) != 1:
+        raise ValueError(f"lora: U / dU must be [M, n_adapters * r] = [{M}, {nA * r}] with contiguous rows")
+    if len(streams) != nA:
+        raise ValueError("lora: one mask stream per adapter")
+    d = _lib.LoraDesc()
+    d.M, d.K, d.r, d.n_adapters = M, K, r, nA
+    d.ldx, d.ldu = x2.stride(0), u2.stride(0)
+    d.scale, d.p = float(scale), float(p)
+    d.seed = int(seed) & (2 ** 64 - 1)
+    for j, s_ in enumerate(streams):
+        d.stream[j] = int(s_)
+    d.accumulate = int(bool(accumulate))
+    return d
+
+
+def lora_down(x: torch.Tensor, A: torch.Tensor, r: int, scale: float, *, p: float = 0.0, seed: int = 0, streams=(0,),
+              out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """U [M, n * r] = scale * (D_j o x) A_j^T for the n = A.shape[0] // r stacked adapters sharing x [M, K]."""
+    _need_cuda(x, A, out)
+    x2 = _rows2d(x)
+    if out is None:
+        out = torch.empty(x2.shape[0], A.shape[0], device=x.device, dtype=BF16)
+    d = _lora_desc(x2, out, A, r, scale, p, seed, streams)
+    _lib.check(_lib.load().u2_lora_down_bf16(x2.data_ptr(), A.data_ptr(), out.data_ptr(), C.byref(d), _stream()),
+               "u2_lora_down_bf16")
+    return out
+
+
+def lora_wgrad(du: torch.Tensor, x: torch.Tensor, dA: torch.Tensor, r: int, scale: float, *, p: float = 0.0, seed: int = 0,
+               streams=(0,), accumulate: bool = False) -> torch.Tensor:
+    """dA_j (+)= scale * dU_j^T (D_j o x) into the stacked gradient dA [n * r, K]."""
+    _need_cuda(du, x, dA)
+    x2 = _rows2d(x)
+    if not dA.is_contiguous():
+        raise ValueError("lora_wgrad: dA must be contiguous")
+    d = _lora_desc(x2, _rows2d(du), dA, r, scale, p, seed, streams, accumulate)
+    _lib.check(_lib.load().u2_lora_wgrad_bf16(du.data_ptr(), x2.data_ptr(), dA.data_ptr(), C.byref(d), _stream()),
+               "u2_lora_wgrad_bf16")
+    return dA
+
+
+def lora_dgrad(du: torch.Tensor, A: torch.Tensor, dx: torch.Tensor, r: int, scale: float, *, p: float = 0.0, seed: int = 0,
+               streams=(0,)) -> torch.Tensor:
+    """dx += sum_j D_j o (scale * dU_j A_j), in place."""
+    _need_cuda(du, A, dx)
+    dx2 = _rows2d(dx)
+    d = _lora_desc(dx2, _rows2d(du), A, r, scale, p, seed, streams)
+    _lib.check(_lib.load().u2_lora_dgrad_bf16(du.data_ptr(), A.data_ptr(), dx2.data_ptr(), C.byref(d), _stream()),
+               "u2_lora_dgrad_bf16")
+    return dx
