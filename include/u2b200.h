@@ -117,8 +117,11 @@ U2_API int u2_rmsnorm_bf16(const void* x, const void* residual, const float* gam
  * Rows are indexed (i0 batch, i1 head in [0,H), i2 query in [0,S)); element strides given for input
  * and output. p[j] = softmax_j(in[j] * scale + rel_bias[(j - i2 + rel_max - 1) * H + i1]) over the
  * visible keys j < n (and j <= i2 + causal_off when causal). Columns [n, zero_pad_to) are written 0.
+ * window > 0 (needs causal): key j is also hidden unless j > i2 + causal_off - window, the sliding-window mask of HF
+ * Phi-3 (transformers masking_utils.py:90-97 sliding_window_overlay `kv_idx > q_idx - sliding_window`, applied through
+ * models/phi3/modeling_phi3.py:265,403); 0 = no window.
  * Replaces F.softmax in rma.py:60-73 (relative bias gather included), tta.py:55-57, the MONAI
- * SABlock softmax and the HF eager attention softmax + causal mask.
+ * SABlock softmax and the HF eager attention softmax + causal (+ sliding-window) mask.
  */
 typedef struct u2_softmax_desc {
   int64_t in_s0, in_s1, in_s2;
@@ -129,6 +132,7 @@ typedef struct u2_softmax_desc {
   int32_t rel_max;
   int32_t causal, causal_off;
   int32_t zero_pad_to;
+  int32_t window;
 } u2_softmax_desc;
 U2_API int u2_softmax_f32_bf16(const float* in, void* out, const u2_softmax_desc* desc, void* stream);
 
@@ -227,6 +231,14 @@ U2_API int u2_decode_attention_bf16(const void* q, const void* k_cache, const vo
                                     int32_t B, int32_t Hq, int32_t Hkv, int32_t dh, int32_t Tmax, int32_t T,
                                     const int32_t* T_dev, int64_t ldq, int64_t ldo, float scale, int32_t T_per_seq,
                                     const int32_t* kv_src, int64_t ld_kv_src, void* stream);
+/* u2_decode_attention_bf16 with a sliding window: sequence b attends keys [max(0, T_b - window), T_b) only and reads
+ * nothing below them (window 0 = no window). The Phi-3 decode step (HF masking_utils.py:90-97, modeling_phi3.py:403).
+ * head_dim 32, 64, 96 or 128 (as u2_decode_attention_bf16). */
+U2_API int u2_decode_attention_window_bf16(const void* q, const void* k_cache, const void* v_cache, void* out,
+                                           int32_t B, int32_t Hq, int32_t Hkv, int32_t dh, int32_t Tmax, int32_t T,
+                                           const int32_t* T_dev, int64_t ldq, int64_t ldo, float scale,
+                                           int32_t T_per_seq, const int32_t* kv_src, int64_t ld_kv_src,
+                                           int32_t window, void* stream);
 
 /* Decode-step linear (weight streaming, HBM-bound): y[b, n] = sum_k norm(x)[b, k] * w[n, k] (+ residual).
  * CUDA-core variant of the HF decoder Linears (+ Qwen3RMSNorm, modeling_qwen3.py:50-67) at q_len == 1 inside generate()
@@ -323,7 +335,8 @@ U2_API int u2_decode_embed_bf16(const int64_t* ids, const void* table, const flo
 
 /* Fused decode-step attention (one launch per layer): per-head RMSNorm (optional) + RoPE of the new q/k,
  * KV-cache append at position pos (or *pos_dev) and GQA attention over the pos + 1 cached keys.
- * qkv [B, (Hq + 2 Hkv) * dh] raw projections; caches [B, Hkv, Tmax, dh]; out [B, Hq * dh].
+ * qkv [B, (Hq + 2 Hkv) * dh] raw projections; caches [B, Hkv, Tmax, dh]; out [B, Hq * dh]. dh 32, 64, 96 or 128
+ * (96: Phi-3-mini; the PV phase runs 24 lanes x 4 elements).
  * Replaces HF modeling_qwen3.py:263-288 at q_len == 1. */
 typedef struct u2_fused_decode_desc {
   int32_t B, Hq, Hkv, dh, Tmax, pos;
@@ -344,6 +357,10 @@ typedef struct u2_fused_decode_desc {
                             t < pos from cache row kv_src[b * ld_kv_src + t] (its new token is always appended to and
                             read from its own row). NULL: every sequence reads its own row (compiled without lookups) */
   int64_t ld_kv_src;     /* >= Tmax when kv_src != NULL */
+  int32_t window;        /* sliding window (Phi-3): attend keys [max(0, pos - window + 1), pos] only, i.e. HF's
+                            `kv_idx > q_idx - sliding_window` (transformers masking_utils.py:90-97, modeling_phi3.py:403);
+                            the split-KV variant deals only the window's 32-key groups to its cluster. 0: no window
+                            (compiled without it). The cache stays full-length: positions index it as before */
 } u2_fused_decode_desc;
 U2_API int u2_decode_attention_fused_bf16(const void* qkv, void* k_cache, void* v_cache, void* out,
                                           const u2_fused_decode_desc* desc, void* stream);

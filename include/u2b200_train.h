@@ -178,6 +178,8 @@ U2_API int u2_cast_bf16_f32(const void* in, float* out, int64_t n, void* stream)
  *   h         = fmix32(fmix32(key_j ^ row) ^ col)                  (row of X in [0, M), column in [0, K))
  *   D_j(row, col) = 0 if h < floor(p * 2^32), else 1 / (1 - p)     (p = 0: every element kept, D = 1)
  * stream[j] names the adapter: the training engine passes layer * 8 + t with t = 0..6 for q, k, v, o, gate, up, down.
+ * Phi-3 (fused HF Phi3 linears, one adapter per call) has its own streams, disjoint from those: 2^24 + layer * 4 + t
+ * with t = 0..3 for qkv_proj, o_proj, gate_up_proj, down_proj.
  * The masked input D_j o X is rounded to bf16 (the dtype PEFT's dropout returns) wherever it is an operand.
  *
  *   u2_lora_down_bf16:  U[:, j] = s * (D_j o X) A_j^T

@@ -47,6 +47,7 @@ class SoftmaxDesc(C.Structure):
         ("rel_max", C.c_int32),
         ("causal", C.c_int32), ("causal_off", C.c_int32),
         ("zero_pad_to", C.c_int32),
+        ("window", C.c_int32),
     ]
 
 
@@ -116,6 +117,7 @@ class FusedDecodeDesc(C.Structure):
         ("kv_splits", C.c_int32), ("pdl", C.c_int32),
         ("pos_per_seq", C.c_int32),
         ("kv_src", C.c_void_p), ("ld_kv_src", C.c_int64),
+        ("window", C.c_int32),
     ]
 
 
@@ -270,6 +272,8 @@ SIGNATURES = {
     "u2_temporal_attention_bf16": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _L, _L, _F, _P, _I, _P]),
     "u2_rope_bf16": (C.c_int, [_P, C.POINTER(RopeDesc), _P]),
     "u2_decode_attention_bf16": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _L, _L, _F, _I, _P, _L, _P]),
+    "u2_decode_attention_window_bf16": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _L, _L, _F, _I, _P, _L,
+                                                  _I, _P]),
     "u2_gemv_bf16": (C.c_int, [_P, _P, _P, C.POINTER(GemvDesc), _P]),
     "u2_argmax_f32": (C.c_int, [_P, _P, _P, _I, _I, _L, _P]),
     "u2_dlinear_bf16": (C.c_int, [_P, _P, _P, C.POINTER(DlinearDesc), _P]),

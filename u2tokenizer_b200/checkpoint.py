@@ -19,7 +19,9 @@ import os
 _FAMILIES = {
     "llama": ("modeling_u2Llama", "u2LlamaForCausalLM", "U2LlamaForCausalLM", "U2LlamaConfig"),
     "qwen3": ("modeling_u2Qwen3", "u2Qwen3ForCausalLM", "U2Qwen3ForCausalLM", "U2Qwen3Config"),
+    "phi3": ("modeling_u2Phi3", "u2Phi3ForCausalLM", "U2Phi3ForCausalLM", "U2Phi3Config"),
 }
+_MODEL_TYPES = {"u2llama": "llama", "u2Qwen3": "qwen3", "u2phi3": "phi3"}
 _CONFIG_STEM, _CONFIG_CLASS = "configuration_u2", "u2Config"
 
 _CONFIG_SHIM = '''"""Remote-code shim: the configuration class of the H100 path under the reference's name
@@ -45,11 +47,9 @@ class {cls}(_Base):
 
 def family_of(config_or_model) -> str:
     mt = getattr(getattr(config_or_model, "config", config_or_model), "model_type", "")
-    if mt == "u2llama":
-        return "llama"
-    if mt == "u2Qwen3":
-        return "qwen3"
-    raise ValueError(f"not a mu2 configuration (model_type={mt!r}; expected 'u2llama' or 'u2Qwen3')")
+    if mt in _MODEL_TYPES:
+        return _MODEL_TYPES[mt]
+    raise ValueError(f"not a mu2 configuration (model_type={mt!r}; expected one of {sorted(_MODEL_TYPES)})")
 
 
 def write_remote_code(directory: str, family: str | None = None) -> dict:
@@ -61,7 +61,7 @@ def write_remote_code(directory: str, family: str | None = None) -> dict:
     with open(cfg_path) as f:
         cfg = json.load(f)
     if family is None:
-        family = {"u2llama": "llama", "u2Qwen3": "qwen3"}.get(cfg.get("model_type"))
+        family = _MODEL_TYPES.get(cfg.get("model_type"))
     if family not in _FAMILIES:
         raise ValueError(f"unknown family {family!r} (config.json model_type={cfg.get('model_type')!r})")
     stem, cls, pkg_cls, pkg_cfg = _FAMILIES[family]

@@ -218,29 +218,38 @@ __device__ __forceinline__ long long kv_src_delta(const int* __restrict__ kv_src
   }
 }
 
-template <int kEpl, bool kInd>  // dh = kEpl * 32: lane owns elements [lane*kEpl, lane*kEpl + kEpl)
+// dh = kEpl * kLanes: lane < kLanes owns elements [lane*kEpl, lane*kEpl + kEpl). dh 96 runs 24 lanes x 4 elements
+// (8-byte accesses; 3 elements per lane would put lanes on 6-byte boundaries); lanes >= kLanes load the last owned
+// slice again, contribute a zero query to the dot products and store nothing.
+// kWin: sliding window of `window` keys (window > 0): only keys [max(0, T - window), T) are read.
+template <int kEpl, bool kInd, bool kWin = false, int kLanes = 32>
 __global__ void __launch_bounds__(256)
 decode_attention_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
                         const __nv_bfloat16* __restrict__ vc, __nv_bfloat16* __restrict__ out, int Hq, int Hkv,
                         int Tmax, int T_host, const int* __restrict__ T_dev, long long ldq, long long ldo,
-                        float scale, int T_per_seq, const int* __restrict__ kv_src, long long ld_src) {
-  constexpr int dh = kEpl * 32;
+                        float scale, int T_per_seq, const int* __restrict__ kv_src, long long ld_src, int window) {
+  constexpr int dh = kEpl * kLanes;
   const int h = blockIdx.x, b = blockIdx.y;
   const int T = T_dev ? min(T_dev[T_per_seq ? b : 0], Tmax) : T_host;
   const int hk = h / (Hq / Hkv);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const __nv_bfloat16* qp = q + (long long)b * ldq + (long long)h * dh + lane * kEpl;
-  const __nv_bfloat16* kp = kc + ((long long)b * Hkv + hk) * Tmax * dh + lane * kEpl;
-  const __nv_bfloat16* vp = vc + ((long long)b * Hkv + hk) * Tmax * dh + lane * kEpl;
+  const bool own = kLanes == 32 || lane < kLanes;
+  const int le = kLanes == 32 ? lane : min(lane, kLanes - 1);
+  const __nv_bfloat16* qp = q + (long long)b * ldq + (long long)h * dh + le * kEpl;
+  const __nv_bfloat16* kp = kc + ((long long)b * Hkv + hk) * Tmax * dh + le * kEpl;
+  const __nv_bfloat16* vp = vc + ((long long)b * Hkv + hk) * Tmax * dh + le * kEpl;
   float qv[kEpl];
   load_epl<kEpl>(qp, qv);
+  const float qs = own ? scale : 0.f;
 #pragma unroll
-  for (int i = 0; i < kEpl; ++i) qv[i] *= scale;
+  for (int i = 0; i < kEpl; ++i) qv[i] *= qs;
   float m = -INFINITY, l = 0.f;
   float acc[kEpl];
 #pragma unroll
   for (int i = 0; i < kEpl; ++i) acc[i] = 0.f;
-  for (int t = warp; t < T; t += 8) {
+  int t_lo = 0;
+  if constexpr (kWin) t_lo = window > 0 ? max(0, T - window) : 0;
+  for (int t = t_lo + warp; t < T; t += 8) {
     float kk[kEpl], vv[kEpl];
     const long long off = (long long)t * dh + kv_src_delta<kInd>(kv_src, ld_src, b, t, T - 1, (long long)Hkv * Tmax * dh);
     load_epl<kEpl>(kp + off, kk);
@@ -263,8 +272,10 @@ decode_attention_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16
     s_m[warp] = m;
     s_l[warp] = l;
   }
+  if (own) {
 #pragma unroll
-  for (int i = 0; i < kEpl; ++i) s_acc[warp][lane * kEpl + i] = acc[i];
+    for (int i = 0; i < kEpl; ++i) s_acc[warp][lane * kEpl + i] = acc[i];
+  }
   __syncthreads();
   float gm = -INFINITY;
 #pragma unroll
@@ -337,29 +348,54 @@ extern "C" U2_API int u2_rope_bf16(void* x, const u2_rope_desc* d, void* stream)
   return U2_OK;
 }
 
-extern "C" U2_API int u2_decode_attention_bf16(const void* q, const void* k_cache, const void* v_cache, void* out,
-                                               int32_t B, int32_t Hq, int32_t Hkv, int32_t dh, int32_t Tmax,
-                                               int32_t T, const int32_t* T_dev, int64_t ldq, int64_t ldo,
-                                               float scale, int32_t T_per_seq, const int32_t* kv_src,
-                                               int64_t ld_kv_src, void* stream) {
+static int decode_attention_launch(const void* q, const void* k_cache, const void* v_cache, void* out, int32_t B,
+                                   int32_t Hq, int32_t Hkv, int32_t dh, int32_t Tmax, int32_t T, const int32_t* T_dev,
+                                   int64_t ldq, int64_t ldo, float scale, int32_t T_per_seq, const int32_t* kv_src,
+                                   int64_t ld_kv_src, int32_t window, void* stream) {
   if (!q || !k_cache || !v_cache || !out) return set_error(U2_ERR_ARG, "decode_attention: null pointer");
   if (Hkv <= 0 || Hq % Hkv) return set_error(U2_ERR_ARG, "decode_attention: Hq must be a multiple of Hkv");
   if (!T_dev && (T <= 0 || T > Tmax)) return set_error(U2_ERR_ARG, "decode_attention: need 0 < T <= Tmax");
   if (T_per_seq && !T_dev) return set_error(U2_ERR_ARG, "decode_attention: T_per_seq needs T_dev");
   if (kv_src && ld_kv_src < Tmax) return set_error(U2_ERR_ARG, "decode_attention: kv_src row stride < Tmax");
+  if (window < 0) return set_error(U2_ERR_ARG, "decode_attention: window %d < 0", window);
   dim3 grid((unsigned)Hq, (unsigned)B);
-#define U2_DA(EPL, IND) decode_attention_kernel<EPL, IND><<<grid, 256, 0, ST(stream)>>>(CBF(q), CBF(k_cache), CBF(v_cache), BF(out), Hq, Hkv, Tmax, T, T_dev, ldq, ldo, scale, T_per_seq != 0, kv_src, ld_kv_src)
-#define U2_DA2(EPL) if (kv_src) U2_DA(EPL, true); else U2_DA(EPL, false)
+#define U2_DA(EPL, IND, WIN, LN) decode_attention_kernel<EPL, IND, WIN, LN><<<grid, 256, 0, ST(stream)>>>(CBF(q), CBF(k_cache), CBF(v_cache), BF(out), Hq, Hkv, Tmax, T, T_dev, ldq, ldo, scale, T_per_seq != 0, kv_src, ld_kv_src, window)
+#define U2_DA2(EPL, LN)                                        \
+  if (window > 0) {                                            \
+    if (kv_src) U2_DA(EPL, true, true, LN);                    \
+    else U2_DA(EPL, false, true, LN);                          \
+  } else if (kv_src) U2_DA(EPL, true, false, LN);              \
+  else U2_DA(EPL, false, false, LN)
   switch (dh) {
-    case 32: U2_DA2(1); break;
-    case 64: U2_DA2(2); break;
-    case 128: U2_DA2(4); break;
-    default: return set_error(U2_ERR_UNSUPPORTED, "decode_attention: head_dim %d (supported: 32, 64, 128)", dh);
+    case 32: U2_DA2(1, 32); break;
+    case 64: U2_DA2(2, 32); break;
+    case 96: U2_DA2(4, 24); break;
+    case 128: U2_DA2(4, 32); break;
+    default: return set_error(U2_ERR_UNSUPPORTED, "decode_attention: head_dim %d (supported: 32, 64, 96, 128)", dh);
   }
 #undef U2_DA2
 #undef U2_DA
   U2_CHECK_LAUNCH("decode_attention");
   return U2_OK;
+}
+
+extern "C" U2_API int u2_decode_attention_bf16(const void* q, const void* k_cache, const void* v_cache, void* out,
+                                               int32_t B, int32_t Hq, int32_t Hkv, int32_t dh, int32_t Tmax,
+                                               int32_t T, const int32_t* T_dev, int64_t ldq, int64_t ldo,
+                                               float scale, int32_t T_per_seq, const int32_t* kv_src,
+                                               int64_t ld_kv_src, void* stream) {
+  return decode_attention_launch(q, k_cache, v_cache, out, B, Hq, Hkv, dh, Tmax, T, T_dev, ldq, ldo, scale, T_per_seq,
+                                 kv_src, ld_kv_src, 0, stream);
+}
+
+extern "C" U2_API int u2_decode_attention_window_bf16(const void* q, const void* k_cache, const void* v_cache,
+                                                      void* out, int32_t B, int32_t Hq, int32_t Hkv, int32_t dh,
+                                                      int32_t Tmax, int32_t T, const int32_t* T_dev, int64_t ldq,
+                                                      int64_t ldo, float scale, int32_t T_per_seq,
+                                                      const int32_t* kv_src, int64_t ld_kv_src, int32_t window,
+                                                      void* stream) {
+  return decode_attention_launch(q, k_cache, v_cache, out, B, Hq, Hkv, dh, Tmax, T, T_dev, ldq, ldo, scale, T_per_seq,
+                                 kv_src, ld_kv_src, window, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -402,8 +438,25 @@ struct FusedDecodeIndArgs : FusedDecodeArgs {
   const int* kv_src;
   long long ld_src;
 };
-template <bool kInd>
-using FusedArgsT = std::conditional_t<kInd, FusedDecodeIndArgs, FusedDecodeArgs>;
+// sliding window (kWin kernels only, with or without the table): keys [max(0, pos - window + 1), pos]
+struct FusedDecodeWinArgs : FusedDecodeIndArgs {
+  int window;
+};
+template <bool kInd, bool kWin = false>
+using FusedArgsT = std::conditional_t<kWin, FusedDecodeWinArgs, std::conditional_t<kInd, FusedDecodeIndArgs, FusedDecodeArgs>>;
+// first visible key of the window (0 without one)
+template <bool kWin>
+__device__ __forceinline__ int window_lo(const FusedArgsT<false, kWin>& a, int pos) {
+  if constexpr (kWin) return a.window > 0 ? max(0, pos - a.window + 1) : 0;
+  else return 0;
+}
+// head_dim elements per lane in the PV phase and the lanes that own them: dh / 32 on 32 lanes, except dh 96 = 24 lanes x
+// 4 elements (8-byte aligned slices); lanes >= kLanes load the last owned slice again and store nothing
+template <int kDh>
+struct PvMap {
+  static constexpr int kEpl = kDh == 96 ? 4 : kDh / 32;
+  static constexpr int kLanes = kDh / kEpl;
+};
 template <bool kInd>
 __device__ __forceinline__ long long kv_src_delta(const FusedArgsT<kInd>& a, int b, int t, int pos, long long row_elems) {
   if constexpr (kInd) return kv_src_delta<true>(a.kv_src, a.ld_src, b, t, pos, row_elems);
@@ -448,18 +501,21 @@ __device__ __forceinline__ void norm_rope_head(const __nv_bfloat16* src, const f
   }
 }
 
-template <int kDh, int kG, bool kInd>
+template <int kDh, int kG, bool kInd, bool kWin = false>
 __global__ void __launch_bounds__(FaCfg<kDh, kG>::kWarps * 32)
-fused_decode_attention_kernel(const FusedArgsT<kInd> a) {
+fused_decode_attention_kernel(const FusedArgsT<kInd, kWin> a) {
   constexpr int kFaWarps = FaCfg<kDh, kG>::kWarps;
-  constexpr int kEpl = kDh / 32;  // head_dim elements per lane in the PV phase
+  constexpr int kEpl = PvMap<kDh>::kEpl;  // head_dim elements per lane in the PV phase
+  constexpr int kLanes = PvMap<kDh>::kLanes;
   constexpr int kPf = 16;         // V rows prefetched per batch (memory-level parallelism in the PV loop)
   const int hk = blockIdx.x, b = blockIdx.y;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int le = kLanes == 32 ? lane : min(lane, kLanes - 1);
   asm volatile("griddepcontrol.wait;" ::: "memory");  // PDL: the QKV projection must have landed
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // o_proj may start prefetching its weights
   const int pos = a.pos_dev ? a.pos_dev[a.pos_per_seq ? b : 0] : a.pos_host;
   const int T = min(pos + 1, a.Tmax);
+  const int lo = window_lo<kWin>(a, pos);  // every 32-key group from lo's group on holds at least one visible key
   __shared__ __align__(16) float s_q[kG][kDh];
   __shared__ float s_m[kFaWarps][kG], s_l[kFaWarps][kG];
   __shared__ float s_acc[kFaWarps][kG][kDh];
@@ -493,14 +549,15 @@ fused_decode_attention_kernel(const FusedArgsT<kInd> a) {
     for (int i = 0; i < kEpl; ++i) acc[g][i] = 0.f;
   }
   const long long row_elems = (long long)a.Hkv * a.Tmax * kDh;
-  for (int t0 = warp * 32; t0 < T; t0 += kFaWarps * 32) {
+  for (int t0 = (lo & ~31) + warp * 32; t0 < T; t0 += kFaWarps * 32) {
     const int t = t0 + lane;
+    const bool vis = t < T && (!kWin || t >= lo);
     // lane's key row (clamped like the V rows below); the V loop takes the other lanes' offsets by shuffle
     const long long dsrc = kv_src_delta<kInd>(a, b, min(t, T - 1), pos, row_elems);
     float s[kG];
 #pragma unroll
     for (int g = 0; g < kG; ++g) s[g] = 0.f;
-    if (t < T) {
+    if (vis) {
       const uint4* kr = reinterpret_cast<const uint4*>(kbase + (long long)t * kDh + dsrc);
       // the whole K row of this lane's key in one burst of independent 16-byte loads (one L2 round trip)
       uint4 u[kDh / 8];
@@ -536,7 +593,7 @@ fused_decode_attention_kernel(const FusedArgsT<kInd> a) {
     for (int g = 0; g < kG; ++g) {
       const float mx = fmaxf(m[g], wmax(s[g]));
       const float corr = __expf(m[g] - mx);
-      p[g] = (t < T) ? __expf(s[g] - mx) : 0.f;
+      p[g] = vis ? __expf(s[g] - mx) : 0.f;
       l[g] = l[g] * corr + wsum(p[g]);
 #pragma unroll
       for (int i = 0; i < kEpl; ++i) acc[g][i] *= corr;
@@ -547,10 +604,10 @@ fused_decode_attention_kernel(const FusedArgsT<kInd> a) {
       float vv[kPf][kEpl];
 #pragma unroll
       for (int jj = 0; jj < kPf; ++jj) {
-        const int tj = min(t0 + j0 + jj, T - 1);  // clamped rows carry probability 0
+        const int tj = min(t0 + j0 + jj, T - 1);  // clamped rows (and rows below the window) carry probability 0
         long long dj = 0;
         if constexpr (kInd) dj = __shfl_sync(0xffffffffu, dsrc, tj - t0);
-        load_epl<kEpl>(vbase + (long long)tj * kDh + dj + lane * kEpl, vv[jj]);
+        load_epl<kEpl>(vbase + (long long)tj * kDh + dj + le * kEpl, vv[jj]);
       }
 #pragma unroll
       for (int jj = 0; jj < kPf; ++jj) {
@@ -570,8 +627,10 @@ fused_decode_attention_kernel(const FusedArgsT<kInd> a) {
       s_m[warp][g] = m[g];
       s_l[warp][g] = l[g];
     }
+    if (kLanes == 32 || lane < kLanes) {
 #pragma unroll
-    for (int i = 0; i < kEpl; ++i) s_acc[warp][g][lane * kEpl + i] = acc[g][i];
+      for (int i = 0; i < kEpl; ++i) s_acc[warp][g][lane * kEpl + i] = acc[g][i];
+    }
   }
   __syncthreads();
   for (int idx = threadIdx.x; idx < kG * kDh; idx += blockDim.x) {
@@ -600,17 +659,19 @@ fused_decode_attention_kernel(const FusedArgsT<kInd> a) {
 // k / v never go through global memory (every CTA recomputes them into shared memory, rank 0 appends them to the
 // cache). CTA partials (m, l, o) are merged by rank 0 over distributed shared memory.
 // ------------------------------------------------------------------------------------------------
-template <int kDh, int kG, bool kInd>
+template <int kDh, int kG, bool kInd, bool kWin = false>
 __global__ void __launch_bounds__(256)
-fused_decode_attention_split_kernel(const FusedArgsT<kInd> a) {
+fused_decode_attention_split_kernel(const FusedArgsT<kInd, kWin> a) {
   namespace cg = cooperative_groups;
   cg::cluster_group cluster = cg::this_cluster();
   constexpr int kW = 8;
-  constexpr int kEpl = kDh / 32;           // head_dim elements per lane in the PV phase
+  constexpr int kEpl = PvMap<kDh>::kEpl;   // head_dim elements per lane in the PV phase
+  constexpr int kLanes = PvMap<kDh>::kLanes;
   constexpr int kVw = (kEpl + 1) / 2;      // 32-bit words holding one V row slice
   const int S = (int)gridDim.z, rank = (int)blockIdx.z;  // the cluster spans the grid's z extent
   const int hk = blockIdx.x, b = blockIdx.y;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int le = kLanes == 32 ? lane : min(lane, kLanes - 1);
   // PDL: the kernel behind us (the next chained decode-linear launch) may start its prologue and weight prefetch
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   // the position is advanced at the end of the previous decode step, several fully serialised launches ago: safe to
@@ -618,6 +679,8 @@ fused_decode_attention_split_kernel(const FusedArgsT<kInd> a) {
   // spans z only), so every CTA of a cluster sees the same T
   const int pos = a.pos_dev ? a.pos_dev[a.pos_per_seq ? b : 0] : a.pos_host;
   const int T = min(pos + 1, a.Tmax);
+  // a window deals only its own key groups (from lo's group on) to the cluster: the bytes read are bounded by it
+  const int lo = window_lo<kWin>(a, pos);
   __shared__ __align__(16) float s_q[kG][kDh];
   __shared__ __align__(16) __nv_bfloat16 s_knew[kDh];
   __shared__ __align__(16) __nv_bfloat16 s_vnew[kDh];
@@ -634,7 +697,7 @@ fused_decode_attention_split_kernel(const FusedArgsT<kInd> a) {
   // A beam-indirection table is written by the previous step's beam kernel, like the positions: safe to read here
   uint4 ku[kDh / 8];
   uint32_t vw[32][kVw];
-  int t0 = (warp * S + rank) * 32;
+  int t0 = (lo & ~31) + (warp * S + rank) * 32;
   const long long row_elems = (long long)a.Hkv * a.Tmax * kDh;
   auto request = [&](int base) {
     const int t = min(base + lane, T - 1);
@@ -647,7 +710,7 @@ fused_decode_attention_split_kernel(const FusedArgsT<kInd> a) {
       const int tj = min(base + jj, T - 1);
       long long dj = 0;
       if constexpr (kInd) dj = __shfl_sync(0xffffffffu, dsrc, tj - base);
-      const __nv_bfloat16* vp = vbase + (long long)tj * kDh + dj + lane * kEpl;
+      const __nv_bfloat16* vp = vbase + (long long)tj * kDh + dj + le * kEpl;
       if constexpr (kEpl == 4) {
         const uint2 u = *reinterpret_cast<const uint2*>(vp);
         vw[jj][0] = u.x;
@@ -721,12 +784,14 @@ fused_decode_attention_split_kernel(const FusedArgsT<kInd> a) {
       }
     }
     float p[kG];
+    const bool vis = t < T && (!kWin || t >= lo);
 #pragma unroll
     for (int g = 0; g < kG; ++g) {
-      if (t >= T) s[g] = -INFINITY;
-      const float mx = fmaxf(m[g], wmax(s[g]));  // lane 0 of every group is a valid key: mx is finite
+      if (!vis) s[g] = -INFINITY;
+      // lane 0 of every group is a valid key (with a window: lane lo & 31 of lo's group): mx is finite
+      const float mx = fmaxf(m[g], wmax(s[g]));
       const float corr = __expf(m[g] - mx);
-      p[g] = (t < T) ? __expf(s[g] - mx) : 0.f;
+      p[g] = vis ? __expf(s[g] - mx) : 0.f;
       l[g] = l[g] * corr + wsum(p[g]);
 #pragma unroll
       for (int i = 0; i < kEpl; ++i) acc[g][i] *= corr;
@@ -737,7 +802,7 @@ fused_decode_attention_split_kernel(const FusedArgsT<kInd> a) {
       float vf[kEpl];
       if (t0 + jj == pos) {  // warp-uniform
 #pragma unroll
-        for (int i = 0; i < kEpl; ++i) vf[i] = __bfloat162float(s_vnew[lane * kEpl + i]);
+        for (int i = 0; i < kEpl; ++i) vf[i] = __bfloat162float(s_vnew[le * kEpl + i]);
       } else if constexpr (kEpl == 4) {
         const float2 x = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&vw[jj][0]));
         const float2 y = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&vw[jj][1]));
@@ -765,8 +830,10 @@ fused_decode_attention_split_kernel(const FusedArgsT<kInd> a) {
       s_m[warp][g] = m[g];
       s_l[warp][g] = l[g];
     }
+    if (kLanes == 32 || lane < kLanes) {
 #pragma unroll
-    for (int i = 0; i < kEpl; ++i) s_acc[warp][g][lane * kEpl + i] = acc[g][i];
+      for (int i = 0; i < kEpl; ++i) s_acc[warp][g][lane * kEpl + i] = acc[g][i];
+    }
   }
   __syncthreads();
   for (int idx = threadIdx.x; idx < kG * kDh; idx += blockDim.x) {
@@ -811,8 +878,8 @@ fused_decode_attention_split_kernel(const FusedArgsT<kInd> a) {
   cluster.sync();  // the other ranks' shared memory must outlive rank 0's reads
 }
 
-template <int kDh, int kG, bool kInd>
-static int launch_fused_decode_split(const FusedArgsT<kInd>& a, dim3 grid, bool pdl, cudaStream_t st) {
+template <int kDh, int kG, bool kInd, bool kWin>
+static int launch_fused_decode_split(const FusedArgsT<kInd, kWin>& a, dim3 grid, bool pdl, cudaStream_t st) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = dim3(256);
@@ -827,35 +894,39 @@ static int launch_fused_decode_split(const FusedArgsT<kInd>& a, dim3 grid, bool 
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 2 : 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, fused_decode_attention_split_kernel<kDh, kG, kInd>, a);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, fused_decode_attention_split_kernel<kDh, kG, kInd, kWin>, a);
   if (e != cudaSuccess) return set_error(U2_ERR_CUDA, "decode_attention_fused (split-KV) launch: %s", cudaGetErrorString(e));
   return U2_OK;
 }
 
-template <int kDh, bool kInd>
-static int launch_fused_decode(const FusedArgsT<kInd>& a, int G, dim3 grid, bool pdl, cudaStream_t st) {
+template <int kDh, bool kInd, bool kWin = false>
+static int launch_fused_decode(const FusedArgsT<kInd, kWin>& a, int G, dim3 grid, bool pdl, cudaStream_t st) {
   if (grid.z > 1) {
     switch (G) {
-      case 1: return launch_fused_decode_split<kDh, 1, kInd>(a, grid, pdl, st);
-      case 2: return launch_fused_decode_split<kDh, 2, kInd>(a, grid, pdl, st);
-      case 4: return launch_fused_decode_split<kDh, 4, kInd>(a, grid, pdl, st);
-      case 8: return launch_fused_decode_split<kDh, 8, kInd>(a, grid, pdl, st);
+      case 1: return launch_fused_decode_split<kDh, 1, kInd, kWin>(a, grid, pdl, st);
+      case 2: return launch_fused_decode_split<kDh, 2, kInd, kWin>(a, grid, pdl, st);
+      case 4: return launch_fused_decode_split<kDh, 4, kInd, kWin>(a, grid, pdl, st);
+      case 8: return launch_fused_decode_split<kDh, 8, kInd, kWin>(a, grid, pdl, st);
       default: return set_error(U2_ERR_UNSUPPORTED, "decode_attention_fused: Hq/Hkv = %d (supported 1, 2, 4, 8)", G);
     }
   }
   switch (G) {
-    case 1: fused_decode_attention_kernel<kDh, 1, kInd><<<grid, FaCfg<kDh, 1>::kWarps * 32, 0, st>>>(a); break;
-    case 2: fused_decode_attention_kernel<kDh, 2, kInd><<<grid, FaCfg<kDh, 2>::kWarps * 32, 0, st>>>(a); break;
-    case 4: fused_decode_attention_kernel<kDh, 4, kInd><<<grid, FaCfg<kDh, 4>::kWarps * 32, 0, st>>>(a); break;
-    case 8: fused_decode_attention_kernel<kDh, 8, kInd><<<grid, FaCfg<kDh, 8>::kWarps * 32, 0, st>>>(a); break;
+    case 1: fused_decode_attention_kernel<kDh, 1, kInd, kWin><<<grid, FaCfg<kDh, 1>::kWarps * 32, 0, st>>>(a); break;
+    case 2: fused_decode_attention_kernel<kDh, 2, kInd, kWin><<<grid, FaCfg<kDh, 2>::kWarps * 32, 0, st>>>(a); break;
+    case 4: fused_decode_attention_kernel<kDh, 4, kInd, kWin><<<grid, FaCfg<kDh, 4>::kWarps * 32, 0, st>>>(a); break;
+    case 8: fused_decode_attention_kernel<kDh, 8, kInd, kWin><<<grid, FaCfg<kDh, 8>::kWarps * 32, 0, st>>>(a); break;
     default: return set_error(U2_ERR_UNSUPPORTED, "decode_attention_fused: Hq/Hkv = %d (supported 1, 2, 4, 8)", G);
   }
   return U2_OK;
 }
 
 template <int kDh>
-static int launch_fused_decode(const FusedDecodeIndArgs& a, int G, dim3 grid, bool pdl, cudaStream_t st) {
-  if (a.kv_src) return launch_fused_decode<kDh, true>(a, G, grid, pdl, st);
+static int launch_fused_decode(const FusedDecodeWinArgs& a, int G, dim3 grid, bool pdl, cudaStream_t st) {
+  if (a.window > 0) {
+    if (a.kv_src) return launch_fused_decode<kDh, true, true>(a, G, grid, pdl, st);
+    return launch_fused_decode<kDh, false, true>(a, G, grid, pdl, st);
+  }
+  if (a.kv_src) return launch_fused_decode<kDh, true>(static_cast<const FusedDecodeIndArgs&>(a), G, grid, pdl, st);
   return launch_fused_decode<kDh, false>(static_cast<const FusedDecodeArgs&>(a), G, grid, pdl, st);
 }
 
@@ -869,7 +940,8 @@ extern "C" U2_API int u2_decode_attention_fused_bf16(const void* qkv, void* k_ca
     return set_error(U2_ERR_UNSUPPORTED, "decode_attention_fused: Hq/Hkv must be an integer <= %d", kFaMaxG);
   if (!d->pos_dev && (d->pos < 0 || d->pos >= d->Tmax)) return set_error(U2_ERR_ARG, "decode_attention_fused: position outside the cache");
   if (d->pos_per_seq && !d->pos_dev) return set_error(U2_ERR_ARG, "decode_attention_fused: pos_per_seq needs pos_dev");
-  FusedDecodeIndArgs a;
+  if (d->window < 0) return set_error(U2_ERR_ARG, "decode_attention_fused: window %d < 0", d->window);
+  FusedDecodeWinArgs a;
   a.qkv = CBF(qkv); a.ldq = d->ldq;
   a.kc = BF(k_cache); a.vc = BF(v_cache);
   a.out = BF(out); a.ldo = d->ldo;
@@ -878,6 +950,7 @@ extern "C" U2_API int u2_decode_attention_fused_bf16(const void* qkv, void* k_ca
   a.q_norm_w = d->q_norm_w; a.k_norm_w = d->k_norm_w; a.eps = d->eps;
   a.inv_freq = d->inv_freq; a.scale = d->scale;
   a.kv_src = d->kv_src; a.ld_src = d->ld_kv_src;
+  a.window = d->window;
   if (a.kv_src && a.ld_src < d->Tmax) return set_error(U2_ERR_ARG, "decode_attention_fused: kv_src row stride < Tmax");
   const int splits = d->kv_splits > 1 ? d->kv_splits : 1;
   if (splits != 1 && splits != 2 && splits != 4 && splits != 8)
@@ -888,8 +961,9 @@ extern "C" U2_API int u2_decode_attention_fused_bf16(const void* qkv, void* k_ca
   switch (d->dh) {
     case 32: rc = launch_fused_decode<32>(a, G, grid, d->pdl != 0, ST(stream)); break;
     case 64: rc = launch_fused_decode<64>(a, G, grid, d->pdl != 0, ST(stream)); break;
+    case 96: rc = launch_fused_decode<96>(a, G, grid, d->pdl != 0, ST(stream)); break;
     case 128: rc = launch_fused_decode<128>(a, G, grid, d->pdl != 0, ST(stream)); break;
-    default: return set_error(U2_ERR_UNSUPPORTED, "decode_attention_fused: head_dim %d (supported 32/64/128)", d->dh);
+    default: return set_error(U2_ERR_UNSUPPORTED, "decode_attention_fused: head_dim %d (supported 32/64/96/128)", d->dh);
   }
   if (rc) return rc;
   U2_CHECK_LAUNCH("decode_attention_fused");

@@ -4,6 +4,8 @@
 #include <cuda_bf16.h>
 #include <math.h>
 
+#include <type_traits>
+
 #include "host_util.h"
 #include "u2b200.h"
 
@@ -168,10 +170,23 @@ struct SoftmaxArgs {
   int causal_off;
   int zero_pad_to;                   // write zeros for columns [n, zero_pad_to)
 };
+// sliding window on top of the causal mask (kWin kernels): key j visible iff j > i + causal_off - window as well
+// (HF masking_utils.sliding_window_overlay, masking_utils.py:90-97, used by Phi-3 through modeling_phi3.py:403).
+// A separate type so that the kernels without a window keep their parameter block and code.
+struct SoftmaxWinArgs : SoftmaxArgs {
+  int window;
+};
+template <bool kWin>
+using SoftmaxArgsT = std::conditional_t<kWin, SoftmaxWinArgs, SoftmaxArgs>;
+template <bool kWin>
+__device__ __forceinline__ int softmax_lo(const SoftmaxArgsT<kWin>& a, int i2) {
+  if constexpr (kWin) return max(0, i2 + a.causal_off - a.window + 1);
+  else return 0;
+}
 
-template <int kGroup, int kMaxV>
+template <int kGroup, int kMaxV, bool kWin = false>
 __global__ void __launch_bounds__(kGroup == 32 ? 128 : kGroup)
-softmax_rows_kernel(const SoftmaxArgs a) {
+softmax_rows_kernel(const SoftmaxArgsT<kWin> a) {
   constexpr int kRowsPerBlock = (kGroup == 32) ? 4 : 1;
   const int gl = threadIdx.x % kGroup;  // lane within the group
   const long long row = (long long)blockIdx.x * kRowsPerBlock + threadIdx.x / kGroup;
@@ -185,6 +200,7 @@ softmax_rows_kernel(const SoftmaxArgs a) {
   const float* in = a.in + i0 * a.in_s0 + i1 * a.in_s1 + i2 * a.in_s2;
   __nv_bfloat16* out = a.out + i0 * a.out_s0 + i1 * a.out_s1 + i2 * a.out_s2;
   const int limit = a.causal ? min(a.n, i2 + a.causal_off + 1) : a.n;  // keys [0, limit) are visible
+  const int lo = softmax_lo<kWin>(a, i2);                                // (keys [lo, limit) with a window)
 
   float v[kMaxV];
   float m = -INFINITY;
@@ -192,7 +208,7 @@ softmax_rows_kernel(const SoftmaxArgs a) {
   for (int i = 0; i < kMaxV; ++i) {
     const int j = i * kGroup + gl;
     float t = -INFINITY;
-    if (active && j < limit) {
+    if (active && j < limit && (!kWin || j >= lo)) {
       t = in[j] * a.scale;
       if (a.rel_bias) t += __ldg(a.rel_bias + (long long)(j - i2 + a.rel_max - 1) * a.H + i1);
     }
@@ -297,8 +313,9 @@ softmax_warp_vec_kernel(const SoftmaxArgs a) {
 
 // Rows longer than the register-resident variants hold (> 8192 keys, e.g. DiffTS over 64 frames x 256 tokens, the
 // reference's own smoke shape svr.py:190-205): one CTA per row, three passes over the (L2-resident) row.
+template <bool kWin = false>
 __global__ void __launch_bounds__(256)
-softmax_long_rows_kernel(const SoftmaxArgs a) {
+softmax_long_rows_kernel(const SoftmaxArgsT<kWin> a) {
   const long long r = blockIdx.x;
   const int i2 = (int)(r % a.S);
   const int i1 = (int)((r / a.S) % a.H);
@@ -306,6 +323,7 @@ softmax_long_rows_kernel(const SoftmaxArgs a) {
   const float* in = a.in + i0 * a.in_s0 + i1 * a.in_s1 + i2 * a.in_s2;
   __nv_bfloat16* out = a.out + i0 * a.out_s0 + i1 * a.out_s1 + i2 * a.out_s2;
   const int limit = a.causal ? min(a.n, i2 + a.causal_off + 1) : a.n;
+  const int lo = softmax_lo<kWin>(a, i2);
   __shared__ float red[8];
   auto score = [&](int j) {
     float t = in[j] * a.scale;
@@ -322,15 +340,15 @@ softmax_long_rows_kernel(const SoftmaxArgs a) {
     return t;
   };
   float m = -INFINITY;
-  for (int j = threadIdx.x; j < limit; j += 256) m = fmaxf(m, score(j));
+  for (int j = lo + threadIdx.x; j < limit; j += 256) m = fmaxf(m, score(j));
   m = block_reduce(m, true);
   float s = 0.f;
-  for (int j = threadIdx.x; j < limit; j += 256) s += __expf(score(j) - m);
+  for (int j = lo + threadIdx.x; j < limit; j += 256) s += __expf(score(j) - m);
   s = block_reduce(s, false);
   const float inv = s > 0.f ? 1.f / s : 0.f;
   const int span = max(a.n, a.zero_pad_to);
   for (int j = threadIdx.x; j < span; j += 256)
-    out[j] = __float2bfloat16(j < limit ? __expf(score(j) - m) * inv : 0.f);
+    out[j] = __float2bfloat16(j < limit && (!kWin || j >= lo) ? __expf(score(j) - m) * inv : 0.f);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -390,7 +408,9 @@ extern "C" U2_API int u2_softmax_f32_bf16(const float* in, void* out, const u2_s
   if (d->n <= 0 || d->n0 <= 0 || d->H <= 0 || d->S <= 0) return set_error(U2_ERR_ARG, "softmax: bad extents");
   if (d->rel_bias && (d->n > d->rel_max || d->S > d->rel_max))
     return set_error(U2_ERR_ARG, "softmax: sequence length %d/%d exceeds the relative-bias table (%d)", d->S, d->n, d->rel_max);
-  SoftmaxArgs a;
+  if (d->window < 0 || (d->window > 0 && !d->causal))
+    return set_error(U2_ERR_ARG, "softmax: window %d needs causal != 0 (and >= 0)", d->window);
+  SoftmaxWinArgs a;
   a.in = in;
   a.out = reinterpret_cast<__nv_bfloat16*>(out);
   a.in_s0 = d->in_s0; a.in_s1 = d->in_s1; a.in_s2 = d->in_s2;
@@ -400,12 +420,18 @@ extern "C" U2_API int u2_softmax_f32_bf16(const float* in, void* out, const u2_s
   a.rel_bias = d->rel_bias; a.rel_max = d->rel_max;
   a.causal = d->causal; a.causal_off = d->causal_off;
   a.zero_pad_to = d->zero_pad_to;
+  a.window = d->window;
+  const bool win = d->window > 0;
+  const SoftmaxArgs& a0 = a;
   const int span = d->n > d->zero_pad_to ? d->n : d->zero_pad_to;
   const long long rows = (long long)d->n0 * d->H * d->S;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-#define U2_SM_CASE(G, MV)                                                                 \
-  softmax_rows_kernel<G, MV><<<(unsigned)((rows + ((G) == 32 ? 4 : 1) - 1) / ((G) == 32 ? 4 : 1)), \
-                               (G) == 32 ? 128 : (G), 0, st>>>(a)
+#define U2_SM_GRID(G) (unsigned)((rows + ((G) == 32 ? 4 : 1) - 1) / ((G) == 32 ? 4 : 1)), (G) == 32 ? 128 : (G), 0, st
+#define U2_SM_CASE(G, MV)                                           \
+  do {                                                              \
+    if (win) softmax_rows_kernel<G, MV, true><<<U2_SM_GRID(G)>>>(a); \
+    else softmax_rows_kernel<G, MV><<<U2_SM_GRID(G)>>>(a0);          \
+  } while (0)
   // long plain rows: warp-per-row vector variant (needs 16-byte aligned fp32 rows, 8-byte aligned bf16 rows, a span that
   // is a whole number of float4 groups - the callers pad rows to 8 elements)
   const bool vec_ok = !d->rel_bias && !d->causal && span > 1024 && span <= 2560 && (span & 3) == 0 &&
@@ -413,7 +439,7 @@ extern "C" U2_API int u2_softmax_f32_bf16(const float* in, void* out, const u2_s
                       (d->out_s1 & 3) == 0 && (d->out_s2 & 3) == 0 && (reinterpret_cast<uintptr_t>(in) & 15) == 0 &&
                       (reinterpret_cast<uintptr_t>(out) & 7) == 0 && d->zero_pad_to >= d->n;
   if (vec_ok) {
-    softmax_warp_vec_kernel<20><<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(a);
+    softmax_warp_vec_kernel<20><<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(a0);
     U2_CHECK_LAUNCH("softmax");
     return U2_OK;
   }
@@ -426,9 +452,11 @@ extern "C" U2_API int u2_softmax_f32_bf16(const float* in, void* out, const u2_s
   else if (span <= 2048) U2_SM_CASE(128, 16);
   else if (span <= 4096) U2_SM_CASE(256, 16);
   else if (span <= 8192) U2_SM_CASE(256, 32);
-  else if (rows <= 0x7fffffffLL) softmax_long_rows_kernel<<<(unsigned)rows, 256, 0, st>>>(a);
+  else if (rows <= 0x7fffffffLL && win) softmax_long_rows_kernel<true><<<(unsigned)rows, 256, 0, st>>>(a);
+  else if (rows <= 0x7fffffffLL) softmax_long_rows_kernel<<<(unsigned)rows, 256, 0, st>>>(a0);
   else return set_error(U2_ERR_UNSUPPORTED, "softmax: %lld rows of length %d", rows, span);
 #undef U2_SM_CASE
+#undef U2_SM_GRID
   U2_CHECK_LAUNCH("softmax");
   return U2_OK;
 }

@@ -10,7 +10,7 @@ gate-up matrices, fp32 vectors) and sequences the kernel launches for
                          TTA (self / visual-cross / text-cross attention, linear aggregation)
                          (reference src/model/u2tokenizer/{u2Tokenizer,svr,tta,rma,rope}.py)
   * the splice         : embed_tokens gather + visual tokens at positions 1..n_vis (u2_arch.py:118-121)
-  * the decoder        : Qwen3 / Llama prefill (tensor-core GEMMs) and KV-cached greedy decode
+  * the decoder        : Qwen3 / Llama / Phi-3 prefill (tensor-core GEMMs) and KV-cached greedy decode
                          (weight-streaming GEMVs), i.e. what HF runs under super().forward()/generate()
 
 All arithmetic happens in hand-written CUDA; torch provides memory, streams and CUDA graphs only.
@@ -244,21 +244,30 @@ class U2Engine:
         g = self.g
         self.embed = t.bf("model.embed_tokens.weight")
         self.layers = []
+        phi3 = g.decoder_family == "phi3"
         for i in range(g.num_hidden_layers):
             l = f"model.layers.{i}."
+            if phi3:
+                # HF Phi3: qkv_proj is already the fused [q; k; v] layout, gate_up_proj is [gate; up] in halves
+                # (modeling_phi3.py:58-62)
+                wqkv = t.bf(l + "self_attn.qkv_proj.weight")
+                gate, up = t.bf(l + "mlp.gate_up_proj.weight").chunk(2, dim=0)
+            else:
+                wqkv = t.cat_bf([l + "self_attn.q_proj.weight", l + "self_attn.k_proj.weight",
+                                 l + "self_attn.v_proj.weight"])
+                gate, up = t.bf(l + "mlp.gate_proj.weight"), t.bf(l + "mlp.up_proj.weight")
             self.layers.append(dict(
                 ln1=t.f32(l + "input_layernorm.weight"),
-                wqkv=t.cat_bf([l + "self_attn.q_proj.weight", l + "self_attn.k_proj.weight",
-                               l + "self_attn.v_proj.weight"]),
+                wqkv=wqkv,
                 qn=t.f32(l + "self_attn.q_norm.weight") if g.qk_norm else None,
                 kn=t.f32(l + "self_attn.k_norm.weight") if g.qk_norm else None,
                 wo=t.bf(l + "self_attn.o_proj.weight"),
                 ln2=t.f32(l + "post_attention_layernorm.weight"),
                 # gate/up rows interleaved (gate_j, up_j) = rows (2j, 2j+1): one copy serves the prefill GEMM
                 # (+ interleaved SiLU*mul) and the decode linear's in-epilogue pairing
-                wgu=torch.stack([t.bf(l + "mlp.gate_proj.weight"), t.bf(l + "mlp.up_proj.weight")], dim=1)
-                .view(2 * g.intermediate_size, g.hidden_size).contiguous(),
+                wgu=torch.stack([gate, up], dim=1).view(2 * g.intermediate_size, g.hidden_size).contiguous(),
                 wdown=t.bf(l + "mlp.down_proj.weight")))
+            del gate, up
         self.final_norm = t.f32("model.norm.weight")
         self.lm_head = self.embed if (g.tie_word_embeddings or not t.has("lm_head.weight")) else t.bf("lm_head.weight")
         self.inv_freq = self._decoder_inv_freq().to(self.dev)
@@ -286,9 +295,10 @@ class U2Engine:
     # attention through the GEMM kernel (scores materialised in fp32, probabilities in bf16)
     # =========================================================================================
     def _attention(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, scale: float,
-                   rel_bias: Optional[torch.Tensor] = None, causal: bool = False):
+                   rel_bias: Optional[torch.Tensor] = None, causal: bool = False, window: int = 0):
         """q [b, Sq, h, dh], k/v [b, Sk, hk, dh] (strided views, dh contiguous), out [b, Sq, h*dh] view.
-        softmax(q k^T * scale (+ rel bias) (+ causal mask)) v, batched over (b, h) on the tensor cores."""
+        softmax(q k^T * scale (+ rel bias) (+ causal mask, + sliding window when window > 0)) v, batched over (b, h) on
+        the tensor cores."""
         b, Sq, h, dh = q.shape
         Sk, hk = k.shape[1], k.shape[2]
         Skp = _pad8(Sk)
@@ -308,7 +318,7 @@ class U2Engine:
                      c_strides=(Sq * Skp, h * Sq * Skp), alpha=scale)
             ops.softmax(sc, pr, n0=nb, H=h, S=Sq, n=Sk, in_strides=(h * Sq * Skp, Sq * Skp, Skp),
                         out_strides=(h * Sq * Skp, Sq * Skp, Skp), rel_bias=rel_bias, rel_max=REL_MAX, causal=causal,
-                        causal_off=Sk - Sq)
+                        causal_off=Sk - Sq, window=window if causal else 0)
             # P @ V with V [Sk, dh] as stored (MN-major B operand): no transposed copy of V
             ops.gemm(pr, vv, oo, M=Sq, N=dh, K=Sk, lda=Skp, ldb=vv.stride(1), ldc=oo.stride(1), zi=h, zo=nb,
                      b_zi_div=h // hk, a_strides=(Sq * Skp, h * Sq * Skp), b_strides=(vv.stride(2), vv.stride(0)),
@@ -595,7 +605,8 @@ class U2Engine:
             ops.rope(qkv, rows=B * L, ld=nqkv, dh=dh, n_q=hq, n_k=hkv, n_v=hkv if cache is not None else 0,
                      inv_freq=self.inv_freq, q_norm_w=w["qn"], k_norm_w=w["kn"], eps=g.rms_norm_eps, pos0=0, pos_div=1,
                      pos_mod=L, k_cache=kc, v_cache=vc, Tmax=cache.max_len if cache is not None else 0, rows_per_batch=L)
-            self._attention(q4[:, :, :hq], q4[:, :, hq:hq + hkv], q4[:, :, hq + hkv:], ctx, 1.0 / math.sqrt(dh), causal=True)
+            self._attention(q4[:, :, :hq], q4[:, :, hq:hq + hkv], q4[:, :, hq + hkv:], ctx, 1.0 / math.sqrt(dh), causal=True,
+                            window=g.window)
             ops.linear(ctx.view(B * L, hq * dh), w["wo"], residual=x, out=x)
             ops.rmsnorm(x, w["ln2"], g.rms_norm_eps, out=y)
             ops.linear(y, w["wgu"], out=gu)
@@ -701,7 +712,8 @@ class U2Engine:
             ops.decode_attention_fused(qkv, cache.k[li], cache.v[li], ctx, B=B, Hq=hq, Hkv=hkv, dh=dh, Tmax=cache.max_len,
                                        inv_freq=self.inv_freq, scale=1.0 / math.sqrt(dh), pos_dev=cache.length_dev,
                                        q_norm_w=w["qn"], k_norm_w=w["kn"], eps=eps, kv_splits=self._kv_splits(B),
-                                       pdl=self.pdl and self.attn_pdl, pos_per_seq=True, kv_src=cache.kv_src)
+                                       pdl=self.pdl and self.attn_pdl, pos_per_seq=True, kv_src=cache.kv_src,
+                                       window=g.window)
             last = li + 1 == nl
             g_next = self.final_norm if last else self.layers[li + 1]["ln1"]
             fl = flags[li] if (self.multi_op and self.fine_deps) else [None] * 4
@@ -823,7 +835,7 @@ class U2Engine:
                      k_cache=cache.k[li], v_cache=cache.v[li], Tmax=cache.max_len, rows_per_batch=1, pos0_per_batch=True)
             ops.decode_attention(qkv, cache.k[li], cache.v[li], ctx, B=B, Hq=hq, Hkv=hkv, dh=dh, Tmax=cache.max_len,
                                  T_dev=cache.length_plus1_dev, ldq=nqkv, ldo=hq * dh, scale=1.0 / math.sqrt(dh),
-                                 T_per_seq=True, kv_src=cache.kv_src)
+                                 T_per_seq=True, kv_src=cache.kv_src, window=g.window)
             ops.gemv(ctx, w["wo"], x, residual=x)
             ops.gemv(x, w["wgu"], act, norm_gamma=w["ln2"], norm_eps=g.rms_norm_eps, silu_pair=True)
             ops.gemv(act, w["wdown"], x, residual=x)

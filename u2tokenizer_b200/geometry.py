@@ -46,8 +46,22 @@ class Geometry:
     rms_norm_eps: float = 1e-6
     rope_theta: float = 1e6
     rope_scaling: Optional[Dict[str, Any]] = None
-    qk_norm: bool = True  # Qwen3: per-head RMSNorm on q,k; Llama: none
+    qk_norm: bool = True  # Qwen3: per-head RMSNorm on q,k; Llama, Phi-3: none
     tie_word_embeddings: bool = False
+    # decoder state-dict naming: "llama" = separate q/k/v_proj and gate/up_proj (Llama and Qwen3), "phi3" = the fused
+    # self_attn.qkv_proj [(hq + 2 hkv) dh, E] and mlp.gate_up_proj [gate; up] of HF Phi3 (modeling_phi3.py:54,58-62)
+    decoder_family: str = "llama"
+    # sliding-window attention (Phi-3): key j is visible from query i iff i - sliding_window < j <= i
+    # (HF masking_utils.sliding_window_overlay); None = unlimited
+    sliding_window: Optional[int] = None
+    # largest of resid_pdrop / embd_pdrop / attention_dropout (Phi-3); eval mode ignores it as HF does, the training
+    # path refuses a non-zero value
+    decoder_dropout: float = 0.0
+
+    @property
+    def window(self) -> int:
+        """The sliding window as the kernels take it: 0 = no window."""
+        return int(self.sliding_window or 0)
 
     # derived
     @property
@@ -83,6 +97,21 @@ class Geometry:
             rs = None
         head_dim = getattr(config, "head_dim", None) or config.hidden_size // config.num_attention_heads
         qk_norm = "qwen3" in config.model_type.lower()
+        family, window, dropout = "llama", None, 0.0
+        if "phi3" in config.model_type.lower():
+            family = "phi3"
+            rope_type = (rs or {}).get("rope_type", (rs or {}).get("type", "default"))
+            if rs is not None:
+                raise NotImplementedError(
+                    f"Phi-3 rope_type {rope_type!r} (longrope / su: Phi-3-mini-128k, Phi-3.5) is not supported: only the "
+                    "default RoPE of the 4k Phi-3 models runs on the CUDA path")
+            prf = float(rp.get("partial_rotary_factor", getattr(config, "partial_rotary_factor", 1.0)) or 1.0)
+            if prf != 1.0:
+                raise NotImplementedError(f"Phi-3 partial_rotary_factor={prf} (Phi-4-mini) is not supported: the CUDA "
+                                          "path rotates the whole head")
+            window = getattr(config, "sliding_window", None)
+            window = int(window) if window else None
+            dropout = max(float(getattr(config, k, 0.0) or 0.0) for k in ("resid_pdrop", "embd_pdrop", "attention_dropout"))
         return cls(
             image_channel=config.image_channel, image_size=list(config.image_size),
             patch_size=list(config.patch_size), vision_select_feature=config.vision_select_feature,
@@ -101,4 +130,5 @@ class Geometry:
             vocab_size=config.vocab_size, rms_norm_eps=config.rms_norm_eps,
             rope_theta=float(rope_theta), rope_scaling=dict(rs) if rs else None, qk_norm=qk_norm,
             tie_word_embeddings=bool(getattr(config, "tie_word_embeddings", False)),
+            decoder_family=family, sliding_window=window, decoder_dropout=dropout,
         )

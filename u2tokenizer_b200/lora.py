@@ -21,9 +21,9 @@ from typing import Optional, Sequence, Union
 import torch
 import torch.nn as nn
 
-from .train import LORA_GROUPS, LORA_TARGETS, LoraSpec
+from .train import LORA_TARGETS, PHI3_LORA_TARGETS, LoraSpec, lora_groups, lora_targets
 
-_TARGET_RE = re.compile(r"model\.layers\.(\d+)\.(self_attn|mlp)\.(" + "|".join(LORA_TARGETS) + r")$")
+_TARGET_RE = re.compile(r"model\.layers\.(\d+)\.(self_attn|mlp)\.(" + "|".join(LORA_TARGETS + PHI3_LORA_TARGETS) + r")$")
 
 
 @dataclass
@@ -92,16 +92,21 @@ def _matches(name: str, targets) -> bool:
 
 
 def _resolve_targets(model: nn.Module, config: LoraConfig):
-    """Names of the modules `config.target_modules` selects; anything but a decoder q/k/v/o/gate/up/down_proj raises."""
+    """Names of the modules `config.target_modules` selects; anything but a decoder q/k/v/o/gate/up/down_proj
+    (Phi-3: qkv/o/gate_up/down_proj) raises."""
     if not config.target_modules:
         raise ValueError("LoraConfig.target_modules must name the modules to adapt (the reference passes "
                          "find_all_linear_names(model))")
     found = [n for n, _ in model.named_modules() if n and _matches(n, config.target_modules)]
     if not found:
         raise ValueError(f"Target modules {config.target_modules} not found in the base model")
+    from .geometry import Geometry
+    g = Geometry.from_hf(model.config)
+    targets = lora_targets(g)
     for n in found:
-        if not _TARGET_RE.fullmatch(n) or not isinstance(model.get_submodule(n), nn.Linear):
-            raise NotImplementedError(f"LoRA on {n!r} is not supported: only the decoder's q/k/v/o/gate/up/down_proj "
+        m = _TARGET_RE.fullmatch(n)
+        if not m or m.group(3) not in targets or not isinstance(model.get_submodule(n), nn.Linear):
+            raise NotImplementedError(f"LoRA on {n!r} is not supported: only the decoder's {'/'.join(targets)} "
                                       "linears can carry adapters")
     layers = {}
     for n in found:
@@ -111,12 +116,12 @@ def _resolve_targets(model: nn.Module, config: LoraConfig):
     n_layers = model.config.num_hidden_layers
     if len(layers) != n_layers or any(v != kinds for v in layers.values()):
         raise NotImplementedError("LoRA targets must be the same projections on every decoder layer")
-    for _, members in LORA_GROUPS:
+    for _, members in lora_groups(g):
         part = kinds.intersection(members)
         if part and len(part) != len(members):
             raise NotImplementedError(f"LoRA on {sorted(part)} without the rest of its fused group {list(members)} is not "
                                       "supported")
-    return found, tuple(t for t in LORA_TARGETS if t in kinds)
+    return found, tuple(t for t in targets if t in kinds)
 
 
 class LoraModel(nn.Module):

@@ -4,6 +4,7 @@ Mirrors the reference classes
 
     u2LlamaForCausalLM(u2MetaForCausalLM, LlamaForCausalLM)   src/model/language_model/u2llama.py:25-142
     u2Qwen3ForCausalLM (Llama-style contract, SURVEY.md F4)    src/model/language_model/u2qwen3.py:25-145
+    u2Phi3ForCausalLM(u2MetaForCausalLM, Phi3ForCausalLM)     src/model/language_model/u2phi3.py:25-140
     u2MetaModel / u2MetaForCausalLM                            src/model/u2_arch.py:10-164
 
 with the same constructor / forward() / generate() / get_model() / initialize_vision_modules() /
@@ -20,11 +21,12 @@ from typing import Any, Dict, List, Optional, Tuple, Union
 import numpy as np
 import torch
 import torch.nn as nn
-from transformers import AutoConfig, AutoModelForCausalLM, LlamaForCausalLM, LlamaModel, Qwen3ForCausalLM, Qwen3Model
+from transformers import (AutoConfig, AutoModelForCausalLM, LlamaForCausalLM, LlamaModel, Phi3ForCausalLM, Phi3Model,
+                          Qwen3ForCausalLM, Qwen3Model)
 from transformers.modeling_outputs import CausalLMOutputWithPast
 
 from . import _lib
-from .configuration import U2LlamaConfig, U2Qwen3Config
+from .configuration import U2LlamaConfig, U2Phi3Config, U2Qwen3Config
 from .geometry import Geometry
 from .synthetic import param_shapes
 
@@ -401,7 +403,7 @@ class U2MetaForCausalLM(ABC):
                               bad_words_ids=words)
         return None if pc.neutral() else pc
 
-    # ---- forward / generate shared by the Llama and Qwen3 wrappers (reference u2llama.py:41-138) ----
+    # ---- forward / generate shared by the Llama, Qwen3 and Phi-3 wrappers (reference u2llama.py:41-138) ----
     def _u2_forward(self, images=None, input_ids=None, labels=None, attention_mask=None, question_ids=None,
                     position_ids=None, past_key_values=None, inputs_embeds=None, use_cache=None,
                     output_attentions=None, output_hidden_states=None, return_dict=None, **kwargs):
@@ -742,14 +744,58 @@ class U2Qwen3ForCausalLM(U2MetaForCausalLM, Qwen3ForCausalLM):
         return out
 
 
+class U2Phi3Model(U2MetaModel, Phi3Model):
+    config_class = U2Phi3Config
+
+    def __init__(self, config):
+        super().__init__(config)
+
+
+class U2Phi3ForCausalLM(U2MetaForCausalLM, Phi3ForCausalLM):
+    """Phi-3 wrapper (reference u2phi3.py:25-140): HF Phi3's fused qkv_proj / gate_up_proj state-dict keys and its
+    sliding window; the decoder runs on the same CUDA engine as the Llama / Qwen3 wrappers."""
+    config_class = U2Phi3Config
+
+    def __init__(self, config):
+        super(Phi3ForCausalLM, self).__init__(config)
+        self.model = U2Phi3Model(config)
+        self.vocab_size = config.vocab_size
+        self.lm_head = nn.Linear(config.hidden_size, config.vocab_size, bias=False)
+        self.post_init()
+
+    def get_model(self):
+        return self.model
+
+    def forward(self, images=None, input_ids=None, labels=None, attention_mask=None, question_ids=None,
+                position_ids=None, past_key_values=None, inputs_embeds=None, use_cache=None, output_attentions=None,
+                output_hidden_states=None, return_dict=None, **kwargs) -> Union[Tuple, CausalLMOutputWithPast]:
+        return self._u2_forward(images, input_ids, labels, attention_mask, question_ids, position_ids, past_key_values,
+                                inputs_embeds, use_cache, output_attentions, output_hidden_states, return_dict, **kwargs)
+
+    @torch.no_grad()
+    def generate(self, images=None, inputs=None, question_ids=None, **kwargs):
+        return self._u2_generate(images, inputs, question_ids, **kwargs)
+
+    def prepare_inputs_for_generation(self, input_ids, past_key_values=None, inputs_embeds=None, **kwargs):
+        images = kwargs.pop("images", None)
+        out = super().prepare_inputs_for_generation(input_ids, past_key_values=past_key_values,
+                                                    inputs_embeds=inputs_embeds, **kwargs)
+        if images is not None:
+            out["images"] = images
+        return out
+
+
 # reference-compatible aliases (class names used by the reference's callers / checkpoints)
 u2LlamaForCausalLM = U2LlamaForCausalLM
 u2Qwen3ForCausalLM = U2Qwen3ForCausalLM
+u2Phi3ForCausalLM = U2Phi3ForCausalLM
 
 
 def register_auto_classes():
-    """AutoConfig / AutoModelForCausalLM registration (reference u2llama.py:141-142, u2qwen3.py:144-145)."""
-    for cfg, mdl in ((U2LlamaConfig, U2LlamaForCausalLM), (U2Qwen3Config, U2Qwen3ForCausalLM)):
+    """AutoConfig / AutoModelForCausalLM registration (reference u2llama.py:141-142, u2qwen3.py:144-145,
+    u2phi3.py:139-140)."""
+    for cfg, mdl in ((U2LlamaConfig, U2LlamaForCausalLM), (U2Qwen3Config, U2Qwen3ForCausalLM),
+                     (U2Phi3Config, U2Phi3ForCausalLM)):
         try:
             AutoConfig.register(cfg.model_type, cfg)
         except ValueError:

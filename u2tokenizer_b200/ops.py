@@ -167,8 +167,9 @@ def rmsnorm(x, gamma, eps=1e-6, residual=None, out=None, sum_out=None):
 
 def softmax(scores: torch.Tensor, out: torch.Tensor, *, n0: int, H: int, S: int, n: int,
             in_strides, out_strides, scale: float = 1.0, rel_bias: Optional[torch.Tensor] = None,
-            rel_max: int = 0, causal: bool = False, causal_off: int = 0, zero_pad_to: int = 0):
-    """fp32 score rows -> bf16 probabilities (see u2_softmax_desc)."""
+            rel_max: int = 0, causal: bool = False, causal_off: int = 0, zero_pad_to: int = 0, window: int = 0):
+    """fp32 score rows -> bf16 probabilities (see u2_softmax_desc). window > 0 (causal only): key j of query i is
+    visible iff i + causal_off - window < j <= i + causal_off (a sliding window; 0 = none)."""
     _need_cuda(scores, out, rel_bias)
     d = _lib.SoftmaxDesc()
     d.in_s0, d.in_s1, d.in_s2 = in_strides
@@ -179,6 +180,7 @@ def softmax(scores: torch.Tensor, out: torch.Tensor, *, n0: int, H: int, S: int,
     d.rel_max = rel_max
     d.causal, d.causal_off = int(causal), causal_off
     d.zero_pad_to = zero_pad_to
+    d.window = int(window or 0)
     _lib.check(_lib.load().u2_softmax_f32_bf16(scores.data_ptr(), out.data_ptr(), C.byref(d), _stream()),
                "u2_softmax_f32_bf16")
     return out
@@ -340,11 +342,18 @@ def rope(x: torch.Tensor, *, rows: int, ld: int, dh: int, n_q: int, n_k: int, n_
 
 def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, out: torch.Tensor, *,
                      B: int, Hq: int, Hkv: int, dh: int, Tmax: int, T: int = 0, T_dev=None, ldq: int, ldo: int,
-                     scale: float, T_per_seq: bool = False, kv_src: Optional[torch.Tensor] = None):
+                     scale: float, T_per_seq: bool = False, kv_src: Optional[torch.Tensor] = None, window: int = 0):
     """T_per_seq: sequence b attends over T_dev[b] keys (int32 [B]).
-    kv_src (beam search): int32 [B, >= Tmax]; key t of sequence b is read from cache row kv_src[b, t]."""
+    kv_src (beam search): int32 [B, >= Tmax]; key t of sequence b is read from cache row kv_src[b, t].
+    window > 0: sliding window, sequence b attends over its last `window` keys only (u2_decode_attention_window_bf16)."""
     _need_cuda(q, k_cache, v_cache, out, T_dev, kv_src)
     _check_kv_src(kv_src, B, Tmax)
+    if window:
+        _lib.check(_lib.load().u2_decode_attention_window_bf16(
+            q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr(), B, Hq, Hkv, dh, Tmax, T, _ptr(T_dev),
+            ldq, ldo, scale, 1 if T_per_seq else 0, _ptr(kv_src), kv_src.stride(0) if kv_src is not None else 0,
+            int(window), _stream()), "u2_decode_attention_window_bf16")
+        return out
     _lib.check(_lib.load().u2_decode_attention_bf16(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                                     out.data_ptr(), B, Hq, Hkv, dh, Tmax, T, _ptr(T_dev), ldq, ldo,
                                                     scale, 1 if T_per_seq else 0, _ptr(kv_src),
@@ -476,8 +485,10 @@ def decode_embed(ids: torch.Tensor, table: torch.Tensor, gamma: torch.Tensor, x:
 def decode_attention_fused(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, out: torch.Tensor, *,
                            B: int, Hq: int, Hkv: int, dh: int, Tmax: int, inv_freq: torch.Tensor, scale: float,
                            pos: int = 0, pos_dev=None, q_norm_w=None, k_norm_w=None, eps: float = 1e-6, kv_splits: int = 1,
-                           pdl: bool = False, pos_per_seq: bool = False, kv_src: Optional[torch.Tensor] = None):
+                           pdl: bool = False, pos_per_seq: bool = False, kv_src: Optional[torch.Tensor] = None,
+                           window: int = 0):
     """q/k norm + RoPE + KV-cache append + GQA attention for one new token per sequence (one launch).
+    window > 0: sliding window, the new token at position pos attends keys [max(0, pos - window + 1), pos] only.
     kv_splits in {2, 4, 8}: a cluster of that many CTAs per (sequence, KV head) splits the cached keys.
     pos_per_seq: sequence b's new token sits at position pos_dev[b] (int32 [B]) instead of pos_dev[0].
     kv_src (beam search): int32 [B, >= Tmax]; the cached key / value t < pos of sequence b is read from cache row
@@ -496,6 +507,7 @@ def decode_attention_fused(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: to
     d.pos_per_seq = 1 if pos_per_seq else 0
     d.kv_src = _ptr(kv_src)
     d.ld_kv_src = kv_src.stride(0) if kv_src is not None else 0
+    d.window = int(window or 0)
     _lib.check(_lib.load().u2_decode_attention_fused_bf16(qkv.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                                           out.data_ptr(), C.byref(d), _stream()),
                "u2_decode_attention_fused_bf16")

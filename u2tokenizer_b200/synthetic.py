@@ -79,16 +79,22 @@ def param_shapes(g: Geometry) -> Dict[str, Tuple[int, ...]]:
     for i in range(g.num_hidden_layers):
         l = f"model.layers.{i}."
         s[l + "input_layernorm.weight"] = (E,)
-        s[l + "self_attn.q_proj.weight"] = (hq * dh, E)
-        s[l + "self_attn.k_proj.weight"] = (hkv * dh, E)
-        s[l + "self_attn.v_proj.weight"] = (hkv * dh, E)
+        if g.decoder_family == "phi3":  # fused projections (HF modeling_phi3.py:54, Phi3Attention.qkv_proj)
+            s[l + "self_attn.qkv_proj.weight"] = ((hq + 2 * hkv) * dh, E)
+        else:
+            s[l + "self_attn.q_proj.weight"] = (hq * dh, E)
+            s[l + "self_attn.k_proj.weight"] = (hkv * dh, E)
+            s[l + "self_attn.v_proj.weight"] = (hkv * dh, E)
         s[l + "self_attn.o_proj.weight"] = (E, hq * dh)
         if g.qk_norm:
             s[l + "self_attn.q_norm.weight"] = (dh,)
             s[l + "self_attn.k_norm.weight"] = (dh,)
         s[l + "post_attention_layernorm.weight"] = (E,)
-        s[l + "mlp.gate_proj.weight"] = (I, E)
-        s[l + "mlp.up_proj.weight"] = (I, E)
+        if g.decoder_family == "phi3":
+            s[l + "mlp.gate_up_proj.weight"] = (2 * I, E)  # [gate; up] in halves
+        else:
+            s[l + "mlp.gate_proj.weight"] = (I, E)
+            s[l + "mlp.up_proj.weight"] = (I, E)
         s[l + "mlp.down_proj.weight"] = (E, I)
     s["model.norm.weight"] = (E,)
     if not g.tie_word_embeddings:

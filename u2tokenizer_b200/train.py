@@ -39,6 +39,27 @@ _VEC_SUFFIX = ("relative_bias", "dynamic_pool.gate_fc.weight", "cls_token", "pos
 LORA_TARGETS = ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj")
 LORA_GROUPS = (("self_attn.", ("q_proj", "k_proj", "v_proj")), ("self_attn.", ("o_proj",)), ("mlp.", ("gate_proj", "up_proj")),
                ("mlp.", ("down_proj",)))
+# Phi-3 (HF Phi3: fused qkv_proj, [gate; up] gate_up_proj): one adapter per group, on the same four fused GEMMs. Its
+# mask streams are PHI3_STREAM_BASE + layer * 4 + index, disjoint from the Llama / Qwen3 streams above
+PHI3_LORA_TARGETS = ("qkv_proj", "o_proj", "gate_up_proj", "down_proj")
+PHI3_LORA_GROUPS = (("self_attn.", ("qkv_proj",)), ("self_attn.", ("o_proj",)), ("mlp.", ("gate_up_proj",)),
+                    ("mlp.", ("down_proj",)))
+PHI3_STREAM_BASE = 1 << 24
+
+
+def lora_targets(g: Geometry) -> Tuple[str, ...]:
+    return PHI3_LORA_TARGETS if g.decoder_family == "phi3" else LORA_TARGETS
+
+
+def lora_groups(g: Geometry):
+    return PHI3_LORA_GROUPS if g.decoder_family == "phi3" else LORA_GROUPS
+
+
+def lora_stream(g: Geometry, layer: int, target: str) -> int:
+    """Dropout-mask stream of one adapter (u2_lora_desc.stream, documented in u2b200_train.h)."""
+    if g.decoder_family == "phi3":
+        return PHI3_STREAM_BASE + layer * 4 + PHI3_LORA_TARGETS.index(target)
+    return layer * 8 + LORA_TARGETS.index(target)
 
 
 @dataclass(frozen=True)
@@ -124,7 +145,7 @@ class Layout:
         first = {}   # base name of a group's first targeted member -> the group's adapter names (A's, then B's)
         skip = set()
         for li in range(g.num_hidden_layers):
-            for pre, members in LORA_GROUPS:
+            for pre, members in lora_groups(g):
                 tg = [t for t in members if t in lora.targets]
                 if not tg:
                     continue
@@ -169,6 +190,10 @@ class TrainEngine:
     def __init__(self, geom: Geometry, state_dict: Dict[str, torch.Tensor], device="cuda", world_size: int = 1, rank: int = 0,
                  group=None, trainable: Optional[Dict[str, bool]] = None, bucket_elems: int = 200_000_000,
                  lora: Optional[LoraSpec] = None):
+        if geom.decoder_dropout:
+            # HF applies resid / embd / attention dropout in train mode (modeling_phi3.py); this path has no dropout
+            raise NotImplementedError(f"training with decoder dropout {geom.decoder_dropout} (Phi-3 resid_pdrop / "
+                                      "embd_pdrop / attention_dropout) is not supported: set them to 0")
         if not torch.cuda.is_available():
             raise RuntimeError("TrainEngine needs a CUDA device: the training path has no CPU implementation")
         from . import _lib
@@ -180,9 +205,9 @@ class TrainEngine:
         self.world, self.rank, self.group = world_size, rank, group
         self.bucket_elems = bucket_elems
         if lora is not None:
-            bad = [t for t in lora.targets if t not in LORA_TARGETS]
+            bad = [t for t in lora.targets if t not in lora_targets(g)]
             if bad or lora.r not in (8, 16, 32, 64) or not 0.0 <= lora.dropout < 1.0:
-                raise NotImplementedError(f"LoRA on the training path: targets in {LORA_TARGETS}, r in (8, 16, 32, 64), "
+                raise NotImplementedError(f"LoRA on the training path: targets in {lora_targets(g)}, r in (8, 16, 32, 64), "
                                           f"0 <= dropout < 1 (got {lora})")
         self.lora = lora
         self.lay = Layout(g, world_size=world_size, bucket_elems=bucket_elems, lora=lora)
@@ -510,9 +535,11 @@ class TrainEngine:
 
     # ---- attention through the GEMM (scores fp32, probabilities bf16 kept for the backward) -----------
     def attention(self, qv: Var, q_view, kv: Var, k_view, vv: Var, v_view, out_shape, scale: float,
-                  rel_name: Optional[str] = None, causal: bool = False, group: str = "u2t", recompute: bool = False) -> Var:
+                  rel_name: Optional[str] = None, causal: bool = False, group: str = "u2t", recompute: bool = False,
+                  window: int = 0) -> Var:
         """q_view / k_view / v_view map the base tensor of a Var (value or gradient, same shape) to the strided 4-D view
-        [b, S, heads, dh]. Returns ctx Var [b, Sq, h*dh] (out_shape may pad the token axis: extra rows stay zero)."""
+        [b, S, heads, dh]. Returns ctx Var [b, Sq, h*dh] (out_shape may pad the token axis: extra rows stay zero).
+        window > 0 (causal only): sliding window in the softmax; the backward needs nothing more, P is 0 outside it."""
         q, k, v = q_view(qv.v), k_view(kv.v), v_view(vv.v)
         b, Sq, h, dh = q.shape
         Sk, hk = k.shape[1], k.shape[2]
@@ -531,7 +558,7 @@ class TrainEngine:
                      c_strides=(Sq * Skp, h * Sq * Skp), alpha=scale)
             ops.softmax(sc, p_, n0=b, H=h, S=Sq, n=Sk, in_strides=(h * Sq * Skp, Sq * Skp, Skp),
                         out_strides=(h * Sq * Skp, Sq * Skp, Skp), rel_bias=rel, rel_max=REL_MAX, causal=causal,
-                        causal_off=Sk - Sq, zero_pad_to=Skp)
+                        causal_off=Sk - Sq, zero_pad_to=Skp, window=window if causal else 0)
             return p_
         saved = {}
         if recompute and dh == 64 and h == hk and rel is None and not causal:
@@ -1000,7 +1027,9 @@ class TrainEngine:
         return out
 
     def decoder(self, x: Var, B: int, Lx: int) -> Var:
-        """Qwen3 / Llama decoder stack (HF modeling_qwen3.py:305-336 per layer), causal, positions 0..L-1 -> final-norm hidden."""
+        """Qwen3 / Llama / Phi-3 decoder stack (HF modeling_qwen3.py:305-336, modeling_phi3.py per layer), causal (+ the
+        Phi-3 sliding window), positions 0..L-1 -> final-norm hidden. Both families run the same four fused GEMMs per layer
+        (q|k|v, o, gate|up in halves, down): Phi-3 stores them as single parameters."""
         g = self.g
         E, hq, hkv, dh, I = g.hidden_size, g.num_attention_heads, g.num_key_value_heads, g.head_dim, g.intermediate_size
         nh = hq + 2 * hkv
@@ -1015,7 +1044,8 @@ class TrainEngine:
             qv = lambda t: t.view(B, Lx, nh, dh)[:, :, :hq]
             kv_ = lambda t: t.view(B, Lx, nh, dh)[:, :, hq:hq + hkv]
             vv_ = lambda t: t.view(B, Lx, nh, dh)[:, :, hq + hkv:]
-            ctx = self.attention(qkv, qv, qkv, kv_, qkv, vv_, (B, Lx, hq * dh), 1.0 / math.sqrt(dh), causal=True, group="dec")
+            ctx = self.attention(qkv, qv, qkv, kv_, qkv, vv_, (B, Lx, hq * dh), 1.0 / math.sqrt(dh), causal=True, group="dec",
+                                 window=g.window)
             c2 = Var(ctx.v.view(B * Lx, hq * dh), ctx.ng)
             self._alias(c2, ctx)
             x = self._dec_linear(c2, li, 1, tr, residual=x)
@@ -1026,10 +1056,10 @@ class TrainEngine:
         return self.rmsnorm(x, "model.norm.weight", "dec", eps)
 
     def _dec_linear(self, x: Var, li: int, gi: int, tr: bool, residual: Optional[Var] = None) -> Var:
-        """Fused group gi of LORA_GROUPS of decoder layer li (q|k|v, o, gate|up, down). Without adapters: one linear
+        """Fused group gi of lora_groups(g) of decoder layer li (q|k|v, o, gate|up, down). Without adapters: one linear
         (wgrad when `tr`). With adapters on (some of) its members: the base output on the frozen weight, then for every
         adapter j  U_j = s (D_j o x) A_j^T (lora_down) and y[:, rows_j] += U_j B_j^T on the GEMM (K = r)."""
-        pre, members = LORA_GROUPS[gi]
+        pre, members = lora_groups(self.g)[gi]
         names = [f"model.layers.{li}.{pre}{t}.weight" for t in members]
         lo = self.lora
         tg = [t for t in members if lo is not None and t in lo.targets]
@@ -1042,7 +1072,7 @@ class TrainEngine:
         an, bn = [a for _, a, _ in trip], [b for _, _, b in trip]
         A, Wb = self.wcat(an), self.wcat(names)
         Bs = [self.w(b) for b in bn]
-        streams = [li * 8 + LORA_TARGETS.index(t) for t in tg]
+        streams = [lora_stream(self.g, li, t) for t in tg]
         p, seed = (lo.dropout, self._lora_seed) if self._lora_seed else (0.0, 0)
         y = ops.linear(x.v, Wb, residual=residual.v if residual is not None else None)
         x2 = x.v.view(-1, x.v.shape[-1])
