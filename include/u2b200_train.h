@@ -148,11 +148,19 @@ typedef struct u2_adamw_desc {
   float lr, beta1, beta2, eps, weight_decay;
   int32_t step;               /* 1-based */
   const float* grad_scale;
+  uint64_t seed;              /* stochastic rounding of bf16 moments (u2_adamw_bf16_mom16); unused with fp32 moments */
+  int64_t index_offset;       /* >= 0: global index of element 0 of this call (ZeRO-1 slice / bucket offset) */
 } u2_adamw_desc;
 U2_API int u2_adamw_bf16(float* master, float* m, float* v, const void* grad, void* param_out, int64_t n,
                          const u2_adamw_desc* desc, void* stream);
 /* same update with bf16 first / second moments (8 instead of 12 bytes of state per parameter: the mode a single GPU
- * needs to hold the whole optimizer state of the 8B model; the sharded multi-GPU step keeps fp32 moments) */
+ * needs to hold the whole optimizer state of the 8B model; the sharded multi-GPU step keeps fp32 moments). The new m
+ * and v are computed in fp32 (and the master update uses those fp32 values), then stored with STOCHASTIC rounding to
+ * bf16: round-to-nearest would freeze v whenever (1 - beta2) |g^2 - v| is below half a bf16 ulp of v (g^2 < ~3 v at
+ * beta2 0.999), so v could only grow and the step size would drift away from fp32 AdamW's. The random bits of element
+ * e are fmix32(fmix32(key ^ lo32(e)) ^ hi32(e)), key = fmix32(lo32(seed) ^ fmix32(hi32(seed) + step * 0x9E3779B9)),
+ * e = index_offset + the element's index in this call; the low 16 bits round m, the high 16 bits round v. Same seed,
+ * step and global index give the same bits, however the buffer is split into calls. */
 U2_API int u2_adamw_bf16_mom16(float* master, void* m, void* v, const void* grad, void* param_out, int64_t n,
                                const u2_adamw_desc* desc, void* stream);
 U2_API int u2_adamw_f32grad(float* master, float* m, float* v, const float* grad, void* param_out_bf16,

@@ -190,6 +190,7 @@ class AdamWDesc(C.Structure):
         ("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float), ("weight_decay", C.c_float),
         ("step", C.c_int32),
         ("grad_scale", C.c_void_p),
+        ("seed", C.c_uint64), ("index_offset", C.c_int64),
     ]
 
 

@@ -930,7 +930,24 @@ dpo_loss_kernel(const float* __restrict__ per_tok, const float* __restrict__ ref
 struct AdamArgs {
   float lr, beta1, beta2, eps, wd, bc1, bc2_rsqrt;
   const float* grad_scale;
+  uint32_t sr_key;      // stochastic rounding of bf16 moments: hash key of (seed, step)
+  long long index0;     // global index of element 0 of this call
 };
+
+// MurmurHash3's fmix32 finaliser: the counter-based hash of the LoRA dropout masks (lora.cu)
+__host__ __device__ __forceinline__ uint32_t adam_fmix32(uint32_t h) {
+  h ^= h >> 16; h *= 0x85EBCA6Bu; h ^= h >> 13; h *= 0xC2B2AE35u; h ^= h >> 16;
+  return h;
+}
+
+// bf16 bits of x rounded stochastically with the 16 random bits r: up (away from zero) with probability
+// (|x| - |trunc(x)|) / ulp, so E[SR(x)] = x. Round-to-nearest would make a moment stall whenever its update is below half
+// a bf16 ulp (v + (1 - beta2)(g^2 - v) with beta2 = 0.999 needs g^2 > ~3 v to move v at all). Inf / NaN round to nearest.
+__device__ __forceinline__ uint32_t bf16_sr_bits(float x, uint32_t r) {
+  const uint32_t u = __float_as_uint(x);
+  if ((u & 0x7F800000u) == 0x7F800000u) return __bfloat16_as_ushort(__float2bfloat16_rn(x));
+  return (u + (r & 0xFFFFu)) >> 16;
+}
 
 __device__ __forceinline__ void ld4(const float* p, long long i, float (&o)[4]) {
   const float4 t = reinterpret_cast<const float4*>(p)[i];
@@ -952,7 +969,10 @@ __device__ __forceinline__ void st4(__nv_bfloat16* p, long long i, const float (
   reinterpret_cast<uint2*>(p)[i] = t;
 }
 
-// fp32 master + bf16 moments (the single-GPU memory mode: 8 instead of 12 bytes of optimizer state per parameter)
+// fp32 master + bf16 moments (the single-GPU memory mode: 8 instead of 12 bytes of optimizer state per parameter).
+// m and v are stored with stochastic rounding; the random bits of element e are fmix32(fmix32(key ^ lo32(e)) ^ hi32(e))
+// with e the GLOBAL index (index0 + local index): its low half rounds m, its high half rounds v. They depend on (seed,
+// step, e) only, so any split of the buffer into calls (ZeRO-1 slices, buckets) stores the same bits.
 __global__ void __launch_bounds__(256)
 adamw_mom16_kernel(float* __restrict__ master, __nv_bfloat16* __restrict__ m, __nv_bfloat16* __restrict__ v,
                    const __nv_bfloat16* __restrict__ grad, __nv_bfloat16* __restrict__ p_bf16, long long n, const AdamArgs a) {
@@ -960,6 +980,7 @@ adamw_mom16_kernel(float* __restrict__ master, __nv_bfloat16* __restrict__ m, __
   const long long nvec = n >> 2;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
     float g[4], w[4], mm[4], vv[4];
+    uint32_t mb[4], vb[4];
     ld4(grad, i, g); ld4(master, i, w); ld4(m, i, mm); ld4(v, i, vv);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -968,8 +989,14 @@ adamw_mom16_kernel(float* __restrict__ master, __nv_bfloat16* __restrict__ m, __
       vv[j] = a.beta2 * vv[j] + (1.f - a.beta2) * gj * gj;
       const float denom = sqrtf(vv[j]) * a.bc2_rsqrt + a.eps;
       w[j] = w[j] * (1.f - a.lr * a.wd) - (a.lr / a.bc1) * (mm[j] / denom);
+      const unsigned long long e = (unsigned long long)(a.index0 + 4 * i + j);
+      const uint32_t h = adam_fmix32(adam_fmix32(a.sr_key ^ (uint32_t)e) ^ (uint32_t)(e >> 32));
+      mb[j] = bf16_sr_bits(mm[j], h);
+      vb[j] = bf16_sr_bits(vv[j], h >> 16);
     }
-    st4(master, i, w); st4(m, i, mm); st4(v, i, vv);
+    st4(master, i, w);
+    reinterpret_cast<uint2*>(m)[i] = make_uint2(mb[0] | (mb[1] << 16), mb[2] | (mb[3] << 16));
+    reinterpret_cast<uint2*>(v)[i] = make_uint2(vb[0] | (vb[1] << 16), vb[2] | (vb[3] << 16));
     if (p_bf16) st4(p_bf16, i, w);
   }
 }
@@ -1333,10 +1360,14 @@ extern "C" U2_API int u2_dpo_loss_f32(const float* per_tok, const float* ref_sum
 
 static int adam_args(const u2_adamw_desc* d, AdamArgs* a) {
   if (!d || d->step < 1) return set_error(U2_ERR_ARG, "adamw: descriptor / step >= 1");
+  if (d->index_offset < 0) return set_error(U2_ERR_ARG, "adamw: index_offset >= 0");
   a->lr = d->lr; a->beta1 = d->beta1; a->beta2 = d->beta2; a->eps = d->eps; a->wd = d->weight_decay;
   a->bc1 = 1.f - powf(d->beta1, (float)d->step);
   a->bc2_rsqrt = 1.f / sqrtf(1.f - powf(d->beta2, (float)d->step));
   a->grad_scale = d->grad_scale;
+  // the LoRA mask's key schedule with the step in place of the stream id
+  a->sr_key = adam_fmix32((uint32_t)d->seed ^ adam_fmix32((uint32_t)(d->seed >> 32) + (uint32_t)d->step * 0x9E3779B9u));
+  a->index0 = d->index_offset;
   return U2_OK;
 }
 

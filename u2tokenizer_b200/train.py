@@ -1373,7 +1373,10 @@ class TrainEngine:
         for i in range(nb):
             lo = i * L.bucket + self.rank * pc
             sl = slice(i * pc, (i + 1) * pc)
-            T.adamw(o["m_master"][sl], o["m_m"][sl], o["m_v"][sl], self._grad_piece(i), self.W[lo:lo + pc], **kw)
+            # index_offset = the slice's offset in the whole matrix region: bf16 moments get the same stochastic rounding
+            # for any world size
+            T.adamw(o["m_master"][sl], o["m_m"][sl], o["m_v"][sl], self._grad_piece(i), self.W[lo:lo + pc], index_offset=lo,
+                    **kw)
             if W_ > 1:
                 # all-gather of the updated slice on the communication stream: it overlaps the remaining AdamW launches and
                 # the NEXT step's forward, which waits per bucket (_wait_params) right before a segment reads its weights

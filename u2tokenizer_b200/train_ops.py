@@ -249,20 +249,24 @@ def dpo_loss(per_tok: torch.Tensor, ref_sum: torch.Tensor, mask: torch.Tensor, b
     return out, coef
 
 
-def _adam_desc(lr, beta1, beta2, eps, weight_decay, step, grad_scale):
+def _adam_desc(lr, beta1, beta2, eps, weight_decay, step, grad_scale, seed, index_offset):
     d = _lib.AdamWDesc()
     d.lr, d.beta1, d.beta2, d.eps, d.weight_decay = lr, beta1, beta2, eps, weight_decay
     d.step = int(step)
     d.grad_scale = _ptr(grad_scale)
+    d.seed = int(seed) & (2 ** 64 - 1)
+    d.index_offset = int(index_offset)
     return d
 
 
 def adamw(master, m, v, grad, param_out, *, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0, step=1, grad_scale=None,
-          param_out_f32=None):
-    """Fused AdamW over a flat shard (torch.optim.AdamW semantics). grad bf16 -> u2_adamw_bf16, fp32 -> u2_adamw_f32grad."""
+          param_out_f32=None, seed=0, index_offset=0):
+    """Fused AdamW over a flat shard (torch.optim.AdamW semantics). grad bf16 -> u2_adamw_bf16, fp32 -> u2_adamw_f32grad;
+    bf16 m / v -> u2_adamw_bf16_mom16, whose stochastic rounding of the moments draws from (seed, step, index_offset +
+    element index)."""
     _need_cuda(master, m, v, grad, param_out, grad_scale, param_out_f32)
     n = master.numel()
-    d = _adam_desc(lr, beta1, beta2, eps, weight_decay, step, grad_scale)
+    d = _adam_desc(lr, beta1, beta2, eps, weight_decay, step, grad_scale, seed, index_offset)
     lib = _lib.load()
     if grad.dtype == BF16 and m.dtype == BF16:
         _lib.check(lib.u2_adamw_bf16_mom16(master.data_ptr(), m.data_ptr(), v.data_ptr(), grad.data_ptr(), _ptr(param_out), n,
