@@ -422,8 +422,8 @@ def _hf_procs(eos, device=DEV):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("family", ["qwen3", "llama"])
-def test_engine_beam_matches_hf_beam_search_on_the_engine_logits(family):
-    from u2tokenizer_b200.engine import BeamSearch, LogitsProcessors, U2Engine
+def test_beam_request_matches_hf_beam_search_on_the_engine_logits(family):
+    from u2tokenizer_b200.engine import BeamSearch, GenerateRequest, LogitsProcessors, U2Engine
     from u2tokenizer_b200.synthetic import synthetic_state_dict
     g, head_kw = _engine_family(family)
     sd16 = synthetic_state_dict(g, seed=3, device="cpu", dtype=torch.bfloat16, **head_kw)
@@ -440,7 +440,7 @@ def test_engine_beam_matches_hf_beam_search_on_the_engine_logits(family):
     compared = total = 0
     for impl in ("tcgen05", "gemv"):
         eng.decode_impl = impl
-        cap = 16 if eng._use_tc_decode(16) else 8
+        cap = eng._decode_rows()
         for use_graph in (False, True):
             for ragged in (True, False):
                 e = emb if ragged else emb[1:2, :lens[1]].contiguous()
@@ -452,16 +452,13 @@ def test_engine_beam_matches_hf_beam_search_on_the_engine_logits(family):
                     bm = BeamSearch(num_beams=K, length_penalty=lp, early_stopping=es, num_return_sequences=n_ret,
                                     pad_token_id=eos[0])
                     lo = []
-                    eng._procs = eng._active(procs)
-                    try:
-                        got = eng._generate_beam(e, n_new, list(eos), use_graph, bm, ln, logits_out=lo)
-                    finally:
-                        eng._procs = None
-                    want = _hf_beam(lo[0], P, K, V, n_new, eos, lp, es, n_ret, procs_kw if procs else {}).cpu()
+                    req = GenerateRequest(n_new, list(eos), processors=procs, beam=bm)
+                    got = eng._generate(e, req, ln, use_graph, logits_out=lo)
+                    want = _hf_beam(lo, P, K, V, n_new, eos, lp, es, n_ret, procs_kw if procs else {}).cpu()
                     # the same selections on the same logits wherever no step of the prompt is a near-tie: HF's
                     # log_softmax and the engine's may differ in the last bit
-                    it = iter(lo[0][1:])
-                    steps, _ = _hf_loop(lo[0][0], lambda par, tok: next(it), P, K, V, n_new, eos, lp, es,
+                    it = iter(lo[1:])
+                    steps, _ = _hf_loop(lo[0], lambda par, tok: next(it), P, K, V, n_new, eos, lp, es,
                                         _hf_procs(eos) if procs else None)
                     got = got.cpu()
                     w = min(got.shape[1], want.shape[1])
@@ -524,7 +521,7 @@ def test_engine_beams_follow_hf_beam_search_over_the_oracle_decoder(family):
                         pad_token_id=eos[0])
         for impl in ("tcgen05", "gemv"):
             eng.decode_impl = impl
-            cap = 16 if eng._use_tc_decode(16) else 8
+            cap = eng._decode_rows()
             for ragged in (True, False):
                 sel = list(range(len(rows))) if ragged else [1]
                 if len(sel) * K > cap:
@@ -558,13 +555,13 @@ def test_engine_beams_follow_hf_beam_search_over_the_oracle_decoder(family):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("family", ["qwen3", "llama"])
-def test_engine_beam_logits_equal_the_oracle_on_each_beams_own_history(family):
+def test_beam_request_logits_equal_the_oracle_on_each_beams_own_history(family):
     """Teacher-forced through the indirection: the logits the engine computes for row k at step t must be the oracle
     decoder's logits for the prompt followed by row k's own history (backtracked from the engine's records). A wrong
     table entry, a table read one step stale or a wrong copy range hands a row another beam's keys / values, which moves
     its logits by far more than the bf16 error."""
     from oracle import u2_oracle as O
-    from u2tokenizer_b200.engine import BeamSearch, U2Engine
+    from u2tokenizer_b200.engine import BeamSearch, GenerateRequest, U2Engine
     from u2tokenizer_b200.synthetic import synthetic_state_dict
     import torch.nn.functional as F
     g, head_kw = _engine_family(family)
@@ -586,8 +583,8 @@ def test_engine_beam_logits_equal_the_oracle_on_each_beams_own_history(family):
             K = 4 if impl == "tcgen05" else 2
             bm = BeamSearch(num_beams=K, length_penalty=1.0, early_stopping="never")
             lo = []
-            eng._generate_beam(emb, n_new, None, use_graph, bm, torch.tensor(lens), logits_out=lo)
-            lo = [x.cpu() for x in lo[0]]
+            eng._generate(emb, GenerateRequest(n_new, beam=bm), torch.tensor(lens), use_graph, logits_out=lo)
+            lo = [x.cpu() for x in lo]
             rec = eng._gen_state["beam"]["rec"].cpu()
             worst, reparented = 0.0, 0
             for t in range(1, len(lo)):

@@ -34,13 +34,14 @@ def processors(vocab):
 
 
 def kernel_us(eng, pc, B, t, launches):
+    from dataclasses import asdict
     from u2tokenizer_b200 import ops
     V = eng.g.vocab_size
     logits = torch.randn(B, V, device="cuda")
     hist = torch.randint(0, 2000, (B, t + 8), device="cuda", dtype=torch.int32)
     ids = hist[:, t - 1].long().contiguous()
     step = torch.full((1,), t, device="cuda", dtype=torch.int32)
-    blk = eng._procs_block(pc)
+    blk = eng._param_block("logits processors", ops.logits_proc_params, V, **asdict(pc))
     run = lambda: ops.logits_process(logits, blk, ids, hist, step_dev=step)
     for _ in range(10):
         run()

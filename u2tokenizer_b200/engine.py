@@ -18,7 +18,7 @@ All arithmetic happens in hand-written CUDA; torch provides memory, streams and 
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass
+from dataclasses import asdict, dataclass, replace
 from typing import Dict, List, Optional, Tuple
 
 import torch
@@ -63,6 +63,50 @@ class BeamSearch:
     early_stopping: object = False
     num_return_sequences: int = 1
     pad_token_id: Optional[int] = None
+
+
+def eos_ids(eos_token_id) -> Tuple[int, ...]:
+    """EOS ids given as None, an int, a list / tuple or a tensor, as a tuple of ints (empty for None)."""
+    if eos_token_id is None:
+        return ()
+    if isinstance(eos_token_id, torch.Tensor):
+        eos_token_id = eos_token_id.reshape(-1).tolist()
+    elif not isinstance(eos_token_id, (list, tuple)):
+        eos_token_id = [eos_token_id]
+    return tuple(int(e) for e in eos_token_id)
+
+
+@dataclass(frozen=True)
+class GenerateRequest:
+    """What the token-picking head of one generate() call does, handed to every decode step of the call.
+    sampling: (temperature, top_k, top_p, seed), or None for greedy argmax. processors: a neutral configuration is kept
+    as None, so it runs exactly as no configuration: no extra launch, the same captured graph. beam: num_beams > 1, or
+    None; with it the sampling is ignored. eos_token_id: anything eos_ids() takes, kept as its tuple."""
+    max_new_tokens: int
+    eos_token_id: Tuple[int, ...] = ()
+    sampling: Optional[Tuple[float, int, float, int]] = None
+    processors: Optional[LogitsProcessors] = None
+    beam: Optional[BeamSearch] = None
+
+    def __post_init__(self):
+        object.__setattr__(self, "eos_token_id", eos_ids(self.eos_token_id))
+        if self.processors is not None and self.processors.neutral():
+            object.__setattr__(self, "processors", None)
+
+
+SEED_STRIDE = 0x9E3779B97F4A7C15
+
+
+def chunk_plan(B: int, n: int, cap: int, beam: bool) -> List[Tuple[torch.Tensor, int]]:
+    """The decode chunks of a generate() call over B prompts with n rows each (row b * n + s is row s of prompt b) when
+    one decode step carries at most cap rows: per chunk, the prompt of each of its rows (CPU int64) and the offset its
+    sampled rows add to the request seed. Beam search takes windows of (cap // n) * n rows, so the beams of a prompt
+    never straddle two chunks; the other modes take windows of cap rows. The sampler keys its random stream by
+    (seed, step, row in the chunk), so multi-sample chunks (n > 1) move the seed by SEED_STRIDE per chunk; the chunks of
+    a batch of one row per prompt all keep the request seed."""
+    width = (cap // n) * n if beam else cap
+    return [(torch.arange(r0, min(B * n, r0 + width)) // n, SEED_STRIDE * ci if n > 1 else 0)
+            for ci, r0 in enumerate(range(0, B * n, width))]
 
 
 class _Take:
@@ -143,15 +187,7 @@ class U2Engine:
         self._prep_decoder(t)
         self._gen_state = None
         self._fwd_state = None
-        self._sampling = None
-        self._samp_dev = None   # 24-byte u2_sample_params block in device memory (read by the captured decode graph)
-        self._samp_host = None
-        self._procs = None      # LogitsProcessors installed for the current generate() call, None when neutral
-        self._lp_dev = None     # its u2_logits_proc_params block in device memory (read by the captured decode graph)
-        self._lp_host = None
-        self._beam = None       # BeamSearch of the current generate() call (num_beams > 1), else None
-        self._beam_dev = None   # its u2_beam_params block in device memory (read by the captured decode graph)
-        self._beam_host = None
+        self._param_blocks = {}  # what -> [host arguments, device block]: see _param_block
         self.last_beam_scores = None  # fp32 [rows] scores of the hypotheses the last beam search returned
 
     # =========================================================================================
@@ -554,6 +590,9 @@ class U2Engine:
             emb = self.multimodal_embeds(ids, im, q)
             return self.lm_logits(self.prefill(emb))
 
+        def capture():
+            st["logits"] = run(st["ids"], st["images"], st["q"])
+
         if not use_graph or st["calls"] < 2:  # the first call runs eagerly (it also configures the kernels' attributes)
             return run(input_ids, images, question_ids)
         if st["graph"] is None:
@@ -561,20 +600,28 @@ class U2Engine:
             st["images"] = images.to(self.dev).clone()
             st["q"] = None if question_ids is None else question_ids.to(self.dev).clone()
             torch.cuda.synchronize()
-            graph = torch.cuda.CUDAGraph()
-            n0 = _lib.launches()
-            with torch.cuda.graph(graph):
-                st["logits"] = run(st["ids"], st["images"], st["q"])
-            st["n"] = _lib.launches() - n0
-            _lib.add_launches(-st["n"])  # capture records, it does not execute
-            st["graph"] = graph
         st["ids"].copy_(input_ids, non_blocking=True)
         st["images"].copy_(images, non_blocking=True)
         if st["q"] is not None:
             st["q"].copy_(question_ids, non_blocking=True)
+        self._replay(st, capture)
+        return st["logits"].clone()
+
+    @staticmethod
+    def _replay(st: dict, capture) -> None:
+        """Replays the CUDA graph st["graph"], recording capture() into it first when it is None. _lib counts kernels as
+        they are launched: a capture records them without running them, so its count (st["n"]) is taken back once and
+        added on every replay."""
+        if st["graph"] is None:
+            graph = torch.cuda.CUDAGraph()
+            n0 = _lib.launches()
+            with torch.cuda.graph(graph):
+                capture()
+            st["n"] = _lib.launches() - n0
+            _lib.add_launches(-st["n"])
+            st["graph"] = graph
         st["graph"].replay()
         _lib.add_launches(st["n"])
-        return st["logits"].clone()
 
     # =========================================================================================
     # decoder: prefill
@@ -691,7 +738,12 @@ class U2Engine:
         dims = (g.hidden_size, g.intermediate_size, g.num_attention_heads * g.head_dim)
         return self.decode_impl == "tcgen05" and B <= 16 and all(k % 64 == 0 for k in dims)
 
-    def decode_step_tc(self, cache: "KVCache") -> torch.Tensor:
+    def _decode_rows(self) -> int:
+        """Sequences one decode step carries: 16 (the dlinear N) on the wgmma path, 8 (the GEMV batch) otherwise."""
+        tc_rows = 16
+        return tc_rows if self._use_tc_decode(tc_rows) else 8
+
+    def decode_step_tc(self, cache: "KVCache", req: Optional[GenerateRequest] = None) -> torch.Tensor:
         """Decode step with every linear on the wgmma stream-K kernel and the RMSNorms folded into its
         epilogues. Launches per step: embed, qkv(0), then per layer [fused attention, one multi-op launch
         o_proj -> gate|up -> down -> next qkv (or lm_head)], argmax  =  2 launches per layer."""
@@ -737,92 +789,74 @@ class U2Engine:
             else:
                 for (xi, wi, yi, kw) in chain:
                     ops.dlinear(xi, wi, yi, pdl=self.pdl, **kw)
-        self._pick_next(logits, ids.view(B), bufs["step"])
+        self._pick_next(logits, ids.view(B), bufs["step"], req)
         cache.advance_device()
         return logits
 
-    def _pick_next(self, logits: torch.Tensor, ids_out: torch.Tensor, step_dev: Optional[torch.Tensor], step: int = 0):
-        """Greedy argmax, or the sampled head (temperature -> top-k -> top-p -> multinomial) when a sampling
-        configuration is active (HF generate(do_sample=True, ...), reference eval/mrg.py:74-75). Installed logits
+    def _pick_next(self, logits: torch.Tensor, ids_out: torch.Tensor, step_dev: Optional[torch.Tensor],
+                   req: Optional[GenerateRequest], step: int = 0):
+        """Greedy argmax (req None: plain argmax), or the sampled head (temperature -> top-k -> top-p -> multinomial)
+        when the request samples (HF generate(do_sample=True, ...), reference eval/mrg.py:74-75). The request's logits
         processors rewrite the logits in place first, from the generation state's history of generated tokens.
         Beam search replaces all of it with the beam step (_beam_pick)."""
-        if self._beam is not None:
-            return self._beam_pick(logits, ids_out, step_dev, step)
-        if self._procs is not None:
-            ops.logits_process(logits, self._procs_block(self._procs), ids_out, self._gen_state["hist"], step=step,
-                               step_dev=step_dev)
-        sp = self._sampling
-        if sp is None:
+        if req is not None and req.beam is not None:
+            return self._beam_pick(logits, ids_out, step_dev, req, step)
+        if req is not None and req.processors is not None:
+            blk = self._param_block("logits processors", ops.logits_proc_params, self.g.vocab_size,
+                                    **asdict(req.processors))
+            ops.logits_process(logits, blk, ids_out, self._gen_state["hist"], step=step, step_dev=step_dev)
+        if req is None or req.sampling is None:
             ops.argmax(logits, ids_out)
         else:
             # parameters (seed included) are read from a device block: the captured decode graph survives a new
             # request's seed / temperature / top-k / top-p
-            ops.sample_dev(logits, self._sampling_block(sp), ids_out, step=step, step_dev=step_dev)
+            ops.sample_dev(logits, self._param_block("sampling parameters", ops.sample_params, *req.sampling), ids_out,
+                           step=step, step_dev=step_dev)
 
-    def _sampling_block(self, sp: dict) -> torch.Tensor:
-        cur = tuple(sorted(sp.items()))
-        if self._samp_dev is None:
-            self._samp_dev = ops.sample_params(self.dev, sp["temperature"], sp["top_k"], sp["top_p"], sp["seed"])
-        elif self._samp_host != cur:
+    def _param_block(self, what: str, make, *args, **kw) -> torch.Tensor:
+        """The device block make(self.dev, *args, **kw) builds (ops.sample_params, logits_proc_params or beam_params),
+        which the decode step reads. A captured decode graph keeps the block's address, so there is one block per
+        `what`, allocated on first use and rewritten in place (make(..., out=block)) only when the arguments change:
+        that is how a new request's values reach the graph without a new capture. A change during a capture would not
+        be recorded, so it is refused."""
+        host = (args, kw)
+        blk = self._param_blocks.get(what)
+        if blk is None:
+            self._param_blocks[what] = blk = [host, make(self.dev, *args, **kw)]
+        elif blk[0] != host:
             if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError("sampling parameters changed inside a CUDA-graph capture")
-            ops.sample_params(self.dev, sp["temperature"], sp["top_k"], sp["top_p"], sp["seed"], out=self._samp_dev)
-        self._samp_host = cur
-        return self._samp_dev
+                raise RuntimeError(f"{what} changed inside a CUDA-graph capture")
+            make(self.dev, *args, out=blk[1], **kw)
+            blk[0] = host
+        return blk[1]
 
-    def _procs_block(self, pc: "LogitsProcessors") -> torch.Tensor:
-        kw = dict(repetition_penalty=pc.repetition_penalty, no_repeat_ngram_size=pc.no_repeat_ngram_size,
-                  min_new_tokens=pc.min_new_tokens, eos_token_ids=pc.eos_token_ids, bad_words_ids=pc.bad_words_ids)
-        if self._lp_dev is None:
-            self._lp_dev = ops.logits_proc_params(self.dev, self.g.vocab_size, **kw)
-        elif self._lp_host != pc:
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError("logits processors changed inside a CUDA-graph capture")
-            ops.logits_proc_params(self.dev, self.g.vocab_size, out=self._lp_dev, **kw)
-        self._lp_host = pc
-        return self._lp_dev
-
-    def _beam_pick(self, logits: torch.Tensor, ids_out: torch.Tensor, step_dev: Optional[torch.Tensor], step: int):
+    def _beam_pick(self, logits: torch.Tensor, ids_out: torch.Tensor, step_dev: Optional[torch.Tensor],
+                   req: GenerateRequest, step: int):
         """HF's beam step: log_softmax -> logits processors (on the log-probs) -> per-row top beams_to_keep of
         log-prob + running score -> per-prompt merge and bookkeeping, which also writes the next ids and reorders the
         cache indirection table and the processor history. logits keeps the raw logits."""
         st = self._gen_state
-        bs = st["beam"]
-        blk = self._beam_block()
+        bs, bm = st["beam"], req.beam
+        blk = self._param_block("beam search parameters", ops.beam_params, num_beams=bm.num_beams,
+                                length_penalty=bm.length_penalty, early_stopping=bm.early_stopping,
+                                max_new_tokens=req.max_new_tokens, eos_token_ids=req.eos_token_id)
         lp = ops.log_softmax(logits, bs["lp"])
-        if self._procs is not None:
-            ops.logits_process(lp, self._procs_block(self._procs), ids_out, st["hist"], step=step, step_dev=step_dev)
+        if req.processors is not None:
+            pblk = self._param_block("logits processors", ops.logits_proc_params, self.g.vocab_size,
+                                     **asdict(req.processors))
+            ops.logits_process(lp, pblk, ids_out, st["hist"], step=step, step_dev=step_dev)
         ops.beam_topk(lp, bs["running"], bs["flags"], blk, bs["cand_val"], bs["cand_tok"])
         ops.beam_step(blk, bs, ids_out, st["cache"].kv_src, st["cache"].length_dev, V=logits.shape[1],
                       hist=st.get("hist"), step=step, step_dev=step_dev)
 
-    def _beam_block(self) -> torch.Tensor:
-        bm, (max_new, eos) = self._beam, self._beam_req
-        cur = (bm.num_beams, float(bm.length_penalty), bm.early_stopping, max_new, eos)
-        kw = dict(num_beams=bm.num_beams, length_penalty=bm.length_penalty, early_stopping=bm.early_stopping,
-                  max_new_tokens=max_new, eos_token_ids=eos)
-        if self._beam_dev is None:
-            self._beam_dev = ops.beam_params(self.dev, **kw)
-        elif self._beam_host != cur:
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError("beam search parameters changed inside a CUDA-graph capture")
-            ops.beam_params(self.dev, out=self._beam_dev, **kw)
-        self._beam_host = cur
-        return self._beam_dev
-
-    @staticmethod
-    def _active(processors: Optional["LogitsProcessors"]) -> Optional["LogitsProcessors"]:
-        """A neutral configuration runs exactly as no configuration: no extra launch, the same captured graph."""
-        return None if processors is None or processors.neutral() else processors
-
-    def decode_step(self, cache: "KVCache") -> torch.Tensor:
+    def decode_step(self, cache: "KVCache", req: Optional[GenerateRequest] = None) -> torch.Tensor:
         """Consumes buffers['ids'] [B,1] (the last token of every sequence), appends sequence b to the cache at
-        position cache.length_dev[b] (read on the device), leaves fp32 logits in buffers['logits'] and the greedy
-        next ids back in buffers['ids']. Launch sequence is CUDA-graph capturable."""
+        position cache.length_dev[b] (read on the device), leaves fp32 logits in buffers['logits'] and the next ids
+        back in buffers['ids'], picked as `req` asks (None: greedy argmax). Launch sequence is CUDA-graph capturable."""
         g = self.g
         B = cache.batch
         if self._use_tc_decode(B):
-            return self.decode_step_tc(cache)
+            return self.decode_step_tc(cache, req)
         hq, hkv, dh = g.num_attention_heads, g.num_key_value_heads, g.head_dim
         bufs = self._decode_buffers(B)
         x, qkv, ctx, act, logits, ids = (bufs[k] for k in ("x", "qkv", "ctx", "act", "logits", "ids"))
@@ -841,12 +875,12 @@ class U2Engine:
             ops.gemv(act, w["wdown"], x, residual=x)
         ops.gemv(x, self.lm_head, logits, norm_gamma=self.final_norm, norm_eps=g.rms_norm_eps)
         bufs["step"] += 1  # the gemv path has no decode_embed kernel to bump the step counter
-        self._pick_next(logits, ids.view(B), bufs["step"])
+        self._pick_next(logits, ids.view(B), bufs["step"], req)
         cache.advance_device()
         return logits
 
     # =========================================================================================
-    # greedy generation (reference u2llama.py:90-127 with do_sample=False)
+    # generation (reference u2llama.py:90-127): greedy, sampled, multi-sample and beam search through one driver
     # =========================================================================================
     @torch.no_grad()
     def generate(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id=None, do_sample: bool = False,
@@ -863,51 +897,110 @@ class U2Engine:
         lengths[b] on, as if it ran alone. None = every prompt fills the whole width.
         beam (num_beams > 1): HF beam search instead of the greedy / sampled pick (do_sample and num_return_sequences are
         then ignored; the beam config carries its own num_return_sequences)."""
+        lens = self._row_lengths(lengths, embeds.shape[0], embeds.shape[1])
         if beam is not None and beam.num_beams > 1:
-            self._sampling = None  # the state key must not carry a previous sampled request's flag
-            self._procs = self._active(processors)
-            try:
-                return self._generate_beam(embeds, max_new_tokens, eos_token_id, use_graph, beam,
-                                           self._row_lengths(lengths, embeds.shape[0], embeds.shape[1]))
-            finally:
-                self._procs = None
-        self._sampling = dict(temperature=float(temperature), top_k=int(top_k or 0), top_p=float(top_p),
-                              seed=int(seed)) if do_sample else None
-        self._procs = self._active(processors)
-        try:
-            lens = self._row_lengths(lengths, embeds.shape[0], embeds.shape[1])
-            if num_return_sequences > 1:
-                return self._generate_multi(embeds, max_new_tokens, eos_token_id, use_graph, int(num_return_sequences),
-                                            lengths=lens)
-            cap = 16 if self._use_tc_decode(16) else 8  # sequences one decode step can carry (dlinear N / gemv batch)
-            if embeds.shape[0] <= cap:
-                return self.generate_greedy(embeds, max_new_tokens, eos_token_id=eos_token_id, use_graph=use_graph,
-                                            lengths=lens)
-            outs = [self.generate_greedy(embeds[b0:b0 + cap].contiguous(), max_new_tokens, eos_token_id=eos_token_id,
-                                         use_graph=use_graph, lengths=lens[b0:b0 + cap])
-                    for b0 in range(0, embeds.shape[0], cap)]
-            width = max(o.shape[1] for o in outs)
-            if any(o.shape[1] != width for o in outs):  # chunks that hit EOS early: pad with EOS (masked by the caller)
-                fill = eos_token_id[0] if isinstance(eos_token_id, (list, tuple)) else eos_token_id
-                outs = [torch.nn.functional.pad(o, (0, width - o.shape[1]), value=int(fill)) for o in outs]
-            return torch.cat(outs, dim=0)
-        finally:
-            self._sampling = None
-            self._procs = None
+            return self._generate(embeds, GenerateRequest(max_new_tokens, eos_token_id, processors=processors,
+                                                          beam=beam), lens, use_graph)
+        sampling = (float(temperature), int(top_k or 0), float(top_p), int(seed)) if do_sample else None
+        req = GenerateRequest(max_new_tokens, eos_token_id, sampling, processors)
+        return self._generate(embeds, req, lens, use_graph, max(1, int(num_return_sequences)))
 
-    def _gen_state_for(self, B: int, cap: int):
+    def generate_greedy(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id=None,
+                        use_graph: bool = True, return_margins: bool = False, force_ids: Optional[torch.Tensor] = None,
+                        logits_out: Optional[list] = None, lengths=None,
+                        processors: Optional[LogitsProcessors] = None):
+        """Prefill on `embeds` [B, L, E], then max_new_tokens greedy decode steps. Returns new ids [B, n] (and the
+        per-step top-1/top-2 logit margins when asked, for margin-aware parity checks). processors: as for generate();
+        the margins and logits_out then hold the processed logits.
+        force_ids [B, n] (parity tests): teacher forcing - the returned ids are still this engine's own picks, but the
+        token fed to the next step is force_ids[:, step], so one near-tie cannot derail the rest of the comparison.
+        logits_out: a list that receives a copy of every step's fp32 logits [B, V].
+        return_margins, force_ids and logits_out need a batch that fits one decode step (_decode_rows()).
+        lengths [B] (optional): prompt b is embeds[b, :lengths[b]]. The prefill runs over the padded width; causal
+        attention keeps the real positions exact, and the cache rows from lengths[b] on are overwritten by the decode
+        steps before any step reads them."""
+        margins = [] if return_margins else None
+        ids = self._generate(embeds, GenerateRequest(max_new_tokens, eos_token_id, processors=processors),
+                             self._row_lengths(lengths, embeds.shape[0], embeds.shape[1]), use_graph,
+                             margins=margins, force_ids=force_ids, logits_out=logits_out)
+        return (ids, torch.stack(margins, dim=1)) if return_margins else ids
+
+    def _generate(self, embeds: torch.Tensor, req: GenerateRequest, lens: torch.Tensor, use_graph: bool = True,
+                  num_return_sequences: int = 1, margins: Optional[list] = None,
+                  force_ids: Optional[torch.Tensor] = None, logits_out: Optional[list] = None) -> torch.Tensor:
+        """The decode driver of every generate() mode. Every prompt gets n rows, num_beams for beam search and
+        num_return_sequences otherwise, decoded in the chunks chunk_plan() lays out over the rows one decode step
+        carries. With n > 1 the prompts are prefilled once and each chunk copies its rows' prompt KV from that cache;
+        with n == 1 each chunk prefills its own prompts straight into its decode cache.
+        lens: the CPU prompt lengths of _row_lengths(). margins / force_ids / logits_out: the hooks of generate_greedy()
+        (logits_out also receives the raw logits of a beam search), for a request that fits one chunk.
+        Greedy and sampled chunks that stop early are padded to the common width with the first EOS id; beam search
+        returns n_ret hypotheses per prompt, best first, filled with HF's fill value (last_beam_scores: their scores)."""
+        B, L, _ = embeds.shape
+        cap, bm, eos = self._decode_rows(), req.beam, req.eos_token_id
+        if bm is not None:
+            K, n_ret = bm.num_beams, bm.num_return_sequences
+            if K > cap:
+                raise ValueError(f"num_beams={K} exceeds the {cap} rows one decode step carries on this path")
+            if not 1 <= n_ret <= K:
+                raise ValueError(f"num_return_sequences={n_ret} must be in 1..num_beams={K}")
+            if len(eos) > _lib.BEAM_MAX_EOS:
+                raise ValueError(f"beam search supports at most {_lib.BEAM_MAX_EOS} EOS ids, got {len(eos)}")
+            fill = (bm.pad_token_id or eos[0]) if eos else -1
+        n = bm.num_beams if bm is not None else num_return_sequences
+        plan = chunk_plan(B, n, cap, bm is not None)
+        if len(plan) > 1 and (margins is not None or force_ids is not None or logits_out is not None):
+            raise ValueError(f"return_margins / force_ids / logits_out need at most {cap} rows, got {B * n}")
+        if n > 1:
+            pc = self.new_cache(B, L)
+            logits0 = self.lm_logits(self._last_hidden(self.prefill(embeds, pc), lens))
+        outs, seqs, scores = [], [], []
+        for src, seed_off in plan:
+            r = req if req.sampling is None else replace(req, sampling=(*req.sampling[:3], req.sampling[3] + seed_off))
+            st = self._gen_state_for(len(src), L + req.max_new_tokens, r)
+            cache = st["cache"]
+            if n > 1:
+                dev_src = src.to(self.dev)
+                cache.k[:, :, :, :L].copy_(pc.k.index_select(1, dev_src))
+                cache.v[:, :, :, :L].copy_(pc.v.index_select(1, dev_src))
+                cache.set_length(lens[src])  # every row continues from its prompt's length
+                chunk_logits0 = logits0.index_select(0, dev_src)
+            else:
+                cache.set_length(0)
+                hidden = self.prefill(embeds[int(src[0]):int(src[-1]) + 1], cache)
+                cache.set_length(lens[src])
+                chunk_logits0 = self.lm_logits(self._last_hidden(hidden, lens[src]))
+            if bm is not None:
+                self._beam_loop(st, chunk_logits0, r, use_graph, logits_out)
+                s, sc = self._beam_backtrack(st["beam"], len(src) // K, K, n_ret, fill)
+                seqs += s
+                scores.append(sc)
+            else:
+                outs.append(self._decode_loop(st, chunk_logits0, r, use_graph, margins, force_ids, logits_out))
+        if bm is not None:
+            out = torch.full((len(seqs), max(len(x) for x in seqs)), fill, dtype=torch.int64)
+            for i, x in enumerate(seqs):
+                out[i, :len(x)] = torch.as_tensor(x, dtype=torch.int64)
+            self.last_beam_scores = torch.cat(scores)
+            return out.to(self.dev)
+        width = max(o.shape[1] for o in outs)
+        if any(o.shape[1] != width for o in outs):  # chunks that hit EOS early: pad with EOS (masked by the caller)
+            outs = [torch.nn.functional.pad(o, (0, width - o.shape[1]), value=eos[0]) for o in outs]
+        return torch.cat(outs, dim=0)
+
+    def _gen_state_for(self, B: int, cap: int, req: GenerateRequest):
         """The static KV cache and the captured decode-step graph are kept across calls with the same (batch, capacity,
         head configuration): capture + instantiation cost ~0.1 s, which would otherwise be paid per request. With logits
         processors the state also holds the history of generated tokens, int32 [B, cap]; with beam search (K > 1) the
         cache's indirection table and the beam buffers of ops.beam_step."""
-        K = self._beam.num_beams if self._beam is not None else 1
-        key = (B, cap, self.decode_impl, self.multi_op, self.fine_deps, self._sampling is not None,
-               self._procs is not None, K)
+        K = req.beam.num_beams if req.beam is not None else 1
+        key = (B, cap, self.decode_impl, self.multi_op, self.fine_deps, req.sampling is not None,
+               req.processors is not None, K)
         st = self._gen_state if (self._gen_state is not None and self._gen_state["key"] == key) else None
         if st is None:
             self._gen_state = None  # drop the old cache before allocating the new one
-            st = dict(key=key, cache=self.new_cache(B, cap), graph=None, n_graph=0)
-            if self._procs is not None:
+            st = dict(key=key, cache=self.new_cache(B, cap), graph=None)
+            if req.processors is not None:
                 st["hist"] = torch.zeros(B, cap, device=self.dev, dtype=torch.int32)
             if K > 1:
                 st["cache"].kv_src = torch.zeros(B, cap, device=self.dev, dtype=torch.int32)
@@ -940,132 +1033,11 @@ class U2Engine:
         B = hidden.shape[0]
         return hidden[torch.arange(B, device=hidden.device), (lens - 1).to(hidden.device)]
 
-    def generate_greedy(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id=None,
-                        use_graph: bool = True, return_margins: bool = False, force_ids: Optional[torch.Tensor] = None,
-                        logits_out: Optional[list] = None, lengths=None,
-                        processors: Optional[LogitsProcessors] = None):
-        """Prefill on `embeds` [B, L, E], then max_new_tokens decode steps (greedy unless a sampling configuration
-        was installed by generate()). Returns new ids [B, n] (and the per-step top-1/top-2 logit margins when
-        asked, for margin-aware parity checks). processors: as for generate() (None keeps what generate() installed);
-        the margins and logits_out then hold the processed logits.
-        force_ids [B, n] (parity tests): teacher forcing - the returned ids are still this engine's own picks, but the
-        token fed to the next step is force_ids[:, step], so one near-tie cannot derail the rest of the comparison.
-        logits_out: a list that receives a copy of every step's fp32 logits [B, V].
-        lengths [B] (optional): prompt b is embeds[b, :lengths[b]]. The prefill runs over the padded width; causal
-        attention keeps the real positions exact, and the cache rows from lengths[b] on are overwritten by the decode
-        steps before any step reads them."""
-        if processors is not None:
-            prev, self._procs = self._procs, self._active(processors)
-            try:
-                return self.generate_greedy(embeds, max_new_tokens, eos_token_id, use_graph, return_margins, force_ids,
-                                            logits_out, lengths)
-            finally:
-                self._procs = prev
-        B, L, _ = embeds.shape
-        lens = self._row_lengths(lengths, B, L)
-        st = self._gen_state_for(B, L + max_new_tokens)
-        cache = st["cache"]
-        cache.set_length(0)
-        hidden = self.prefill(embeds, cache)
-        cache.set_length(lens)
-        logits0 = self.lm_logits(self._last_hidden(hidden, lens))
-        return self._decode_loop(st, logits0, max_new_tokens, eos_token_id, use_graph, return_margins,
-                                 force_ids=force_ids, logits_out=logits_out)
-
-    def _generate_multi(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id, use_graph: bool, n: int,
-                        lengths=None, processors: Optional[LogitsProcessors] = None):
-        if processors is not None:
-            prev, self._procs = self._procs, self._active(processors)
-            try:
-                return self._generate_multi(embeds, max_new_tokens, eos_token_id, use_graph, n, lengths)
-            finally:
-                self._procs = prev
-        B, L, _ = embeds.shape
-        lens = self._row_lengths(lengths, B, L)
-        pc = self.new_cache(B, L)
-        hidden = self.prefill(embeds, pc)
-        logits0 = self.lm_logits(self._last_hidden(hidden, lens))
-        rows = B * n
-        chunk = 16 if self._use_tc_decode(16) else 8  # sequences one decode step can carry (dlinear N / gemv batch)
-        base = dict(self._sampling) if self._sampling else None
-        outs = []
-        for ci, c0 in enumerate(range(0, rows, chunk)):
-            src_cpu = torch.arange(c0, min(rows, c0 + chunk)) // n  # prompt of every row of this chunk
-            src = src_cpu.to(self.dev)
-            if base is not None:  # distinct random streams per chunk (the sampler keys its stream by (seed, step, row))
-                self._sampling = dict(base, seed=(base["seed"] + 0x9E3779B97F4A7C15 * ci) & ((1 << 64) - 1))
-            st = self._gen_state_for(int(src.numel()), L + max_new_tokens)
-            cache = st["cache"]
-            cache.k[:, :, :, :L].copy_(pc.k.index_select(1, src))
-            cache.v[:, :, :, :L].copy_(pc.v.index_select(1, src))
-            cache.set_length(lens.index_select(0, src_cpu))  # every sample continues from its prompt's length
-            outs.append(self._decode_loop(st, logits0.index_select(0, src), max_new_tokens, eos_token_id, use_graph, False))
-        width = max(o.shape[1] for o in outs)
-        if any(o.shape[1] != width for o in outs):  # chunks that hit EOS early: pad with EOS (masked by the caller)
-            fill = eos_token_id[0] if isinstance(eos_token_id, (list, tuple)) else eos_token_id
-            outs = [torch.nn.functional.pad(o, (0, width - o.shape[1]), value=int(fill)) for o in outs]
-        return torch.cat(outs, dim=0)
-
-    def _generate_beam(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id, use_graph: bool,
-                       beam: BeamSearch, lens: torch.Tensor, logits_out: Optional[list] = None) -> torch.Tensor:
-        """Beam search over B prompts: one prefill, the prompt KV replicated into the K beam rows of every prompt (as
-        _generate_multi does), then chunks of cap // K prompts per decode batch. Returns [B * num_return_sequences, n]
-        ids, best hypothesis first per prompt, cropped to the longest returned one and filled with HF's fill value.
-        logits_out (tests): receives every step's raw fp32 logits [rows, V] of each chunk, a list per chunk."""
-        K, n_ret = int(beam.num_beams), int(beam.num_return_sequences)
-        cap = 16 if self._use_tc_decode(16) else 8  # sequences one decode step can carry (dlinear N / gemv batch)
-        if K > cap:
-            raise ValueError(f"num_beams={K} exceeds the {cap} rows one decode step carries on this path")
-        if not 1 <= n_ret <= K:
-            raise ValueError(f"num_return_sequences={n_ret} must be in 1..num_beams={K}")
-        if eos_token_id is None:
-            eos = ()
-        elif isinstance(eos_token_id, torch.Tensor):
-            eos = tuple(int(e) for e in eos_token_id.reshape(-1).tolist())
-        else:
-            eos = tuple(int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id]))
-        if len(eos) > _lib.BEAM_MAX_EOS:
-            raise ValueError(f"beam search supports at most {_lib.BEAM_MAX_EOS} EOS ids, got {len(eos)}")
-        fill = (beam.pad_token_id or eos[0]) if eos else -1
-        B, L, _ = embeds.shape
-        pc = self.new_cache(B, L)
-        hidden = self.prefill(embeds, pc)
-        logits0 = self.lm_logits(self._last_hidden(hidden, lens))
-        per = cap // K
-        self._beam, self._beam_req = beam, (int(max_new_tokens), eos)
-        seqs, scores = [], []
-        try:
-            for p0 in range(0, B, per):
-                P = min(per, B - p0)
-                src_cpu = torch.arange(p0 * K, (p0 + P) * K) // K  # prompt of every beam row
-                src = src_cpu.to(self.dev)
-                st = self._gen_state_for(P * K, L + max_new_tokens)
-                cache = st["cache"]
-                cache.k[:, :, :, :L].copy_(pc.k.index_select(1, src))
-                cache.v[:, :, :, :L].copy_(pc.v.index_select(1, src))
-                cache.set_length(lens.index_select(0, src_cpu))
-                lo = None
-                if logits_out is not None:
-                    lo = []
-                    logits_out.append(lo)
-                self._beam_loop(st, logits0.index_select(0, src), max_new_tokens, use_graph, lo)
-                s, sc = self._beam_backtrack(st["beam"], P, K, n_ret, fill)
-                seqs += s
-                scores.append(sc)
-        finally:
-            self._beam = None
-        width = max(len(x) for x in seqs)
-        out = torch.full((len(seqs), width), fill, dtype=torch.int64)
-        for i, x in enumerate(seqs):
-            out[i, :len(x)] = torch.as_tensor(x, dtype=torch.int64)
-        self.last_beam_scores = torch.cat(scores)
-        return out.to(self.dev)
-
-    def _beam_loop(self, st, logits0: torch.Tensor, max_new_tokens: int, use_graph: bool, logits_out: Optional[list]):
+    def _beam_loop(self, st, logits0: torch.Tensor, req: GenerateRequest, use_graph: bool, logits_out: Optional[list]):
         """The first beam step on the prefill logits, then up to max_new_tokens - 1 decode steps (the steps after the
         first replay one captured graph); every 16 steps the host checks whether every prompt is done."""
         cache, bs = st["cache"], st["beam"]
-        R, K = cache.batch, self._beam.num_beams
+        R, K = cache.batch, req.beam.num_beams
         bufs = self._decode_buffers(R)
         self.reset_decode_state(R)
         bs["running"].view(-1, K).fill_(-1e9)[:, 0] = 0.0
@@ -1073,26 +1045,16 @@ class U2Engine:
         bs["fin_info"].copy_(torch.tensor([0, -1, 0, 0], dtype=torch.int32).expand(R, 4))
         bs["flags"].copy_(torch.tensor([1, 0], dtype=torch.int32).expand(R // K, 2))
         cache.kv_src.copy_(torch.arange(R, device=self.dev, dtype=torch.int32)[:, None].expand(R, cache.max_len))
-        self._pick_next(logits0, bufs["ids"].view(R), None, step=0)
+        self._pick_next(logits0, bufs["ids"].view(R), None, req, step=0)
         if logits_out is not None:
             logits_out.append(logits0.float().clone())
-        graph, n_graph = st["graph"], st["n_graph"]
-        for step in range(1, max_new_tokens):
+        for step in range(1, req.max_new_tokens):
             if step % 16 == 1 and bool(bs["flags"][:, 1].all()):
                 break
-            if use_graph and (graph is not None or step >= 2):
-                if graph is None:
-                    n0 = _lib.launches()
-                    graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(graph):
-                        self.decode_step(cache)
-                    n_graph = _lib.launches() - n0
-                    _lib.add_launches(-n_graph)  # capture records, it does not execute
-                    st["graph"], st["n_graph"] = graph, n_graph
-                graph.replay()
-                _lib.add_launches(n_graph)
+            if use_graph and (st["graph"] is not None or step >= 2):
+                self._replay(st, lambda: self.decode_step(cache, req))
             else:
-                self.decode_step(cache)
+                self.decode_step(cache, req)
             if logits_out is not None:
                 logits_out.append(bufs["logits"].clone())
 
@@ -1117,57 +1079,39 @@ class U2Engine:
                 keep.append(r)
         return seqs, score[keep]
 
-    def _decode_loop(self, st, logits0: torch.Tensor, max_new_tokens: int, eos_token_id, use_graph: bool,
-                     return_margins: bool, force_ids: Optional[torch.Tensor] = None, logits_out: Optional[list] = None):
+    def _decode_loop(self, st, logits0: torch.Tensor, req: GenerateRequest, use_graph: bool,
+                     margins: Optional[list] = None, force_ids: Optional[torch.Tensor] = None,
+                     logits_out: Optional[list] = None):
         """Pick the first token from `logits0`, then run max_new_tokens - 1 decode steps on st['cache'] (whose length
-        is the prompt length); the steps after the first replay one captured CUDA graph."""
-        from . import _lib
+        is the prompt length); the steps after the first replay one captured CUDA graph. margins: a list that receives
+        every step's top-1/top-2 logit margins [B] (the steps then run eagerly)."""
         cache = st["cache"]
         B = cache.batch
         bufs = self._decode_buffers(B)
         self.reset_decode_state(B)
-        out = torch.empty(B, max_new_tokens, device=self.dev, dtype=torch.int64)
-        margins = []
-        self._pick_next(logits0, bufs["ids"].view(B), None, step=0)
+        out = torch.empty(B, req.max_new_tokens, device=self.dev, dtype=torch.int64)
+        self._pick_next(logits0, bufs["ids"].view(B), None, req, step=0)
         out[:, 0] = bufs["ids"].view(B)
         if logits_out is not None:
             logits_out.append(logits0.float().clone())
         if force_ids is not None:
             force_ids = force_ids.to(self.dev, torch.int64)
             bufs["ids"].view(B).copy_(force_ids[:, 0])
-        if return_margins:
+        if margins is not None:
             t2 = logits0.topk(2, dim=-1).values
             margins.append(t2[:, 0] - t2[:, 1])
-        eos = None
-        if eos_token_id is not None:
-            eos = torch.as_tensor(eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id],
-                                  device=self.dev)
+        eos = torch.as_tensor(req.eos_token_id, device=self.dev) if req.eos_token_id else None
         n_done = 1
-        graph = st["graph"]
-        n_graph = st["n_graph"]
-
-        def finished() -> bool:
-            return eos is not None and bool(torch.isin(out[:, :n_done], eos).any(dim=1).all())
-
-        for step in range(1, max_new_tokens):
-            if eos is not None and (step % 16 == 1) and finished():
+        for step in range(1, req.max_new_tokens):
+            if eos is not None and (step % 16 == 1) and bool(torch.isin(out[:, :n_done], eos).any(dim=1).all()):
                 break
-            if use_graph and not return_margins and (graph is not None or step >= 2):
-                if graph is None:
-                    # step 1 ran eagerly (warm-up + validation of the launch sequence); capture the same
-                    # sequence once - positions are read from the device, so every replay is a new step
-                    n0 = _lib.launches()
-                    graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(graph):
-                        self.decode_step(cache)
-                    n_graph = _lib.launches() - n0
-                    _lib.add_launches(-n_graph)  # capture records, it does not execute
-                    st["graph"], st["n_graph"] = graph, n_graph
-                graph.replay()
-                _lib.add_launches(n_graph)
+            if use_graph and margins is None and (st["graph"] is not None or step >= 2):
+                # step 1 ran eagerly (warm-up + validation of the launch sequence); capture the same
+                # sequence once - positions are read from the device, so every replay is a new step
+                self._replay(st, lambda: self.decode_step(cache, req))
             else:
-                lg = self.decode_step(cache)
-                if return_margins:
+                lg = self.decode_step(cache, req)
+                if margins is not None:
                     t2 = lg.topk(2, dim=-1).values
                     margins.append(t2[:, 0] - t2[:, 1])
             out[:, step] = bufs["ids"].view(B)
@@ -1176,11 +1120,7 @@ class U2Engine:
             if force_ids is not None:
                 bufs["ids"].view(B).copy_(force_ids[:, step])
             n_done += 1
-        res = out[:, :n_done]
-        if return_margins:
-            return res, torch.stack(margins, dim=1)
-        return res
-
+        return out[:, :n_done]
 
 class KVCache:
     """Static KV cache [layers][B, Hkv, Tmax, dh] bf16 + the current length of every sequence on the device

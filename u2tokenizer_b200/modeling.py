@@ -343,7 +343,7 @@ class U2MetaForCausalLM(ABC):
         only; min_length counts from the padded prompt width (max(min_length - prompt_width, 0) new tokens) and
         min_new_tokens takes precedence over it; without an EOS id min_new_tokens has nothing to ban. bad_words_ids is
         validated as NoBadWordsLogitsProcessor does, and one-token words equal to an EOS id are dropped first."""
-        from .engine import LogitsProcessors
+        from .engine import LogitsProcessors, eos_ids
 
         def opt(name):
             v = kwargs.pop(name, None)
@@ -366,12 +366,7 @@ class U2MetaForCausalLM(ABC):
         min_len = count("min_length", opt("min_length"))
         if min_new is None:
             min_new = max((min_len or 0) - int(prompt_width), 0)
-        if eos_token_id is None:
-            eos = []
-        elif isinstance(eos_token_id, torch.Tensor):
-            eos = [int(e) for e in eos_token_id.reshape(-1).tolist()]
-        else:
-            eos = [int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])]
+        eos = eos_ids(eos_token_id)
         bad = opt("bad_words_ids")
         words = ()
         if bad is not None:
@@ -526,9 +521,9 @@ class U2MetaForCausalLM(ABC):
         if max_new is None:
             max_len = kwargs.pop("max_length", None) or (gc.max_length if gc is not None else 20)
             max_new = max(1, max_len - L)
+        from .engine import eos_ids
         eos = kwargs.pop("eos_token_id", None)
-        if eos is None and gc is not None:
-            eos = gc.eos_token_id
+        eos = eos_ids(gc.eos_token_id if eos is None and gc is not None else eos)
         pad = kwargs.pop("pad_token_id", None)
         if pad is None and gc is not None:
             pad = gc.pad_token_id
@@ -545,12 +540,11 @@ class U2MetaForCausalLM(ABC):
                            num_return_sequences=n_ret, lengths=lengths, processors=procs, beam=beam)
         if beam is not None:
             return ids  # HF's beam output: best hypotheses first, each filled after its end with pad or eos[0]
-        if eos is not None:
-            eos_t = torch.as_tensor(eos if isinstance(eos, (list, tuple)) else [eos], device=ids.device)
-            hit = torch.isin(ids, eos_t)
+        if eos:
+            hit = torch.isin(ids, torch.as_tensor(eos, device=ids.device))
             after = (hit.cumsum(dim=1) - hit.long()) > 0  # strictly after the first EOS
             if pad is None:
-                pad = int(eos_t[0])
+                pad = eos[0]
             ids = ids.masked_fill(after, pad)
             keep = int((~after).any(dim=0).sum())
             ids = ids[:, :max(keep, 1)]
