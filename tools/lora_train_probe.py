@@ -6,7 +6,12 @@ Reports peak torch.cuda.max_memory_allocated, the step time (CUDA events, after 
 kernels in a separate torch.profiler run, with the card name and power limit read in the same process. A batch that
 does not fit is reported as such and the next smaller one is tried.
 
-    python tools/lora_train_probe.py --moments fp32 [--out results.json]
+--checkpoint on runs the step with activation checkpointing (TrainEngine(checkpoint=True), what
+gradient_checkpointing_enable() turns on); --checkpoint both runs the plain and the checkpointed step alternately on the
+same engine and reports each (a mode that runs out of memory is reported as not fitting; the batch falls back only when
+neither fits).
+
+    python tools/lora_train_probe.py --moments fp32 [--seq 1024] [--checkpoint both] [--out results.json]
 
 The result is printed as one JSON line; --out also writes it to a file.
 """
@@ -57,7 +62,7 @@ def batch(g, B, frames, seq, n_question, lt):
     return [t.cuda() for t in (images, ids, qids, labels)]
 
 
-def run(B, args):
+def run(B, args, modes):
     from u2tokenizer_b200.configuration import QWEN3_8B, U2Qwen3Config
     from u2tokenizer_b200.geometry import Geometry
     from u2tokenizer_b200.synthetic import synthetic_state_dict
@@ -76,38 +81,59 @@ def run(B, args):
     data = batch(g, B, 8, args.seq, 32, 512)
     torch.manual_seed(0)
 
-    def step():
+    def step(ck):
+        te.checkpoint = ck
         te.zero_grad()
         loss = te.forward_backward(*data)
         te.optimizer_step()
         return loss
-    for _ in range(args.warmup):
-        step()
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats()
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(args.steps + 1)]
-    ev[0].record()
-    for i in range(args.steps):
-        loss = step()
-        ev[i + 1].record()
-    torch.cuda.synchronize()
-    times = [ev[i].elapsed_time(ev[i + 1]) for i in range(args.steps)]
-    peak = torch.cuda.max_memory_allocated()
+    out = {}
+    fit = []
+    for ck in modes:
+        try:
+            for _ in range(args.warmup):
+                step(ck)
+            torch.cuda.synchronize()
+            fit.append(ck)
+        except torch.cuda.OutOfMemoryError as e:
+            te.tape = []
+            out[ck] = dict(batch=B, checkpoint=ck, fits=False, error=str(e).splitlines()[0])
+            import gc
+            gc.collect()
+            torch.cuda.empty_cache()
+    if not fit:
+        return None, list(out.values())
+    times, peaks, loss = {ck: [] for ck in fit}, {ck: 0 for ck in fit}, {}
+    for _ in range(args.steps):
+        for ck in fit:   # the modes alternate step by step: clock and neighbour drift hit both alike
+            torch.cuda.synchronize()
+            torch.cuda.reset_peak_memory_stats()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            loss[ck] = step(ck)
+            e1.record()
+            torch.cuda.synchronize()
+            times[ck].append(e0.elapsed_time(e1))
+            peaks[ck] = max(peaks[ck], torch.cuda.max_memory_allocated())
     from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        step()
-        torch.cuda.synchronize()
-    tot = lora = 0.0
-    for e in prof.key_averages():
-        t = e.device_time_total if hasattr(e, "device_time_total") else e.cuda_time_total
-        if e.device_type is not None and "cpu" in str(e.device_type).lower():
-            continue
-        tot += t
-        if "lora_" in e.key:
-            lora += t
-    return dict(batch=B, fits=True, loss=float(loss), step_ms_median=sorted(times)[len(times) // 2], step_ms=times,
-                peak_alloc_gib=peak / 2 ** 30, frozen_gib=L.frozen_total * 2 / 2 ** 30, trainable_params=n_train,
-                gm_gib=L.mat_total * 2 / 2 ** 30, lora_kernel_share=lora / max(tot, 1e-9), kernel_time_ms=tot / 1e3)
+    for ck in fit:
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            step(ck)
+            torch.cuda.synchronize()
+        tot = lora = 0.0
+        for e in prof.key_averages():
+            t = e.device_time_total if hasattr(e, "device_time_total") else e.cuda_time_total
+            if e.device_type is not None and "cpu" in str(e.device_type).lower():
+                continue
+            tot += t
+            if "lora_" in e.key:
+                lora += t
+        ts = times[ck]
+        out[ck] = dict(batch=B, checkpoint=ck, fits=True, loss=float(loss[ck]), step_ms_median=sorted(ts)[len(ts) // 2],
+                       step_ms=ts, peak_alloc_gib=peaks[ck] / 2 ** 30, frozen_gib=L.frozen_total * 2 / 2 ** 30,
+                       trainable_params=n_train, gm_gib=L.mat_total * 2 / 2 ** 30, lora_kernel_share=lora / max(tot, 1e-9),
+                       kernel_time_ms=tot / 1e3)
+    return fit, [out[ck] for ck in modes if ck in out]
 
 
 def main():
@@ -117,25 +143,26 @@ def main():
     ap.add_argument("--seq", type=int, default=512)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--checkpoint", choices=("off", "on", "both"), default="off",
+                    help="activation checkpointing of the training tape; both: plain and checkpointed steps alternately")
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("lora_train_probe needs a CUDA device")
+    modes = {"off": [False], "on": [True], "both": [False, True]}[args.checkpoint]
     res = dict(card=card(), moments=args.moments, seq=args.seq, runs=[])
     t0 = time.time()
     for B in range(args.batch, 0, -1):
         try:
-            r = run(B, args)
+            fit, runs = run(B, args, modes)
         except torch.cuda.OutOfMemoryError as e:
-            res["runs"].append(dict(batch=B, fits=False, error=str(e).splitlines()[0]))
-            r = None
-        if r is None:
-            import gc
-            gc.collect()
-            torch.cuda.empty_cache()
-            continue
-        res["runs"].append(r)
-        break
+            fit, runs = None, [dict(batch=B, fits=False, error=str(e).splitlines()[0])]
+        res["runs"].extend(runs)
+        import gc
+        gc.collect()
+        torch.cuda.empty_cache()
+        if fit:
+            break
     res["wall_s"] = time.time() - t0
     if args.out:
         Path(args.out).parent.mkdir(parents=True, exist_ok=True)

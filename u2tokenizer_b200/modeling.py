@@ -415,6 +415,9 @@ class U2MetaForCausalLM(ABC):
             # saved activations on the training engine, backward through ONE autograd node that hands every parameter its
             # gradient (computed by the hand-written backward pass, not by torch autograd)
             te = self.train_engine()
+            # gradient_checkpointing_enable() / _disable() set HF's per-module flags; the training tape honours them by
+            # recomputing every repeated block in the backward (TrainEngine._segment), from this step on
+            te.checkpoint = self.is_gradient_checkpointing
             names, params = zip(*[(n, p) for n, p in self.named_parameters() if p.requires_grad])
             loss = _U2TrainLoss.apply(te, (images, input_ids, question_ids, labels), names, *params)
             if return_dict is False:

@@ -5,7 +5,9 @@ config/ds_config.json:27-39; src/train/dpo_u2trainer.py:185-359 for stage 2) is 
 
   * `TrainEngine.forward_backward(...)`  - vision tower -> projector -> mu2-tokenizer -> splice -> decoder -> loss head,
     every activation the backward needs kept in HBM, then the backward pass: dgrad / wgrad and the attention
-    contractions on the wgmma GEMM (transposed operands, no copies), everything else on train_kernels.cu;
+    contractions on the wgmma GEMM (transposed operands, no copies), everything else on train_kernels.cu; with
+    `checkpoint` set (HF gradient_checkpointing_enable()) every repeated block keeps only its input and output and is
+    recomputed in the backward (`_segment`);
   * flat parameter / gradient buffers in a TRAINING LAYOUT (q|k|v, gate|up, wk|wv adjacent, so that one GEMM produces the
     fused gradient; every reference parameter is a contiguous slice, the nn.Parameters of the HF-style module are
     re-pointed at those slices);
@@ -18,6 +20,7 @@ No arithmetic in torch: torch provides memory, streams, NCCL. There is no CPU pa
 """
 from __future__ import annotations
 
+import functools
 import math
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -189,7 +192,7 @@ class Var:
 class TrainEngine:
     def __init__(self, geom: Geometry, state_dict: Dict[str, torch.Tensor], device="cuda", world_size: int = 1, rank: int = 0,
                  group=None, trainable: Optional[Dict[str, bool]] = None, bucket_elems: int = 200_000_000,
-                 lora: Optional[LoraSpec] = None):
+                 lora: Optional[LoraSpec] = None, checkpoint: bool = False):
         if geom.decoder_dropout:
             # HF applies resid / embd / attention dropout in train mode (modeling_phi3.py); this path has no dropout
             raise NotImplementedError(f"training with decoder dropout {geom.decoder_dropout} (Phi-3 resid_pdrop / "
@@ -250,6 +253,11 @@ class TrainEngine:
         self._gm_offs = sorted((L.mat_off[n], n) for n in L.mat_names)
         self._gm_names_cache = {}
         self._lora_seed = 0   # dropout-mask seed of the current forward (0 with p = 0 or outside a training forward)
+        # activation checkpointing (HF gradient_checkpointing_enable()): every repeated block of the training tape keeps
+        # only its input and output and is recomputed in the backward (see _segment). Read at the start of each training
+        # forward; _ckpt is the value the current tape was built with
+        self.checkpoint = bool(checkpoint)
+        self._ckpt = False
 
     # =========================================================================================
     # flat-buffer views
@@ -437,6 +445,37 @@ class TrainEngine:
                             self.comm_stream.wait_event(ev)
                             self.reduce_bucket(b)
         self.tape.append(done)
+
+    def _segment(self, body, x: Var) -> Var:
+        """One repeated block (ViT block, SVR layer, TTA layer, decoder layer): out = body(x), body starting with the
+        block's _mark. Plain: body's ops go on the tape. Checkpointed: body runs on a local tape that is dropped at once
+        (the block's intermediates are freed; only x and out stay alive), and the tape gets one entry that, in the
+        backward, runs body(x) again on the same input Vars - same weight views, kernels and arguments, and the LoRA
+        dropout seed of this forward, so every value is bit-identical - hands out's gradient to the recomputed output and
+        runs the local tape in reverse. External inputs the body closes over (the TTA layers' vis / t_tokens) receive
+        their contributions in the plain order, and the block's marker still fires right after its last wgrad."""
+        if not self._ckpt:
+            return body(x)
+        outer, seed = self.tape, self._lora_seed
+        self.tape = []
+        try:
+            out = body(x)
+        finally:
+            self.tape = outer
+
+        def bwd():
+            outer_, seed_ = self.tape, self._lora_seed
+            self.tape, self._lora_seed = [], seed
+            try:
+                out2 = body(x)
+                local = self.tape
+            finally:
+                self.tape, self._lora_seed = outer_, seed_
+            out2.g, out.g = out.g, None
+            for fn in reversed(local):
+                fn()
+        self.tape.append(bwd)
+        return out
 
     # ---- linear ---------------------------------------------------------------------------------
     def linear(self, x: Var, w: torch.Tensor, gw: Optional[torch.Tensor], bias: Optional[torch.Tensor] = None,
@@ -701,7 +740,8 @@ class TrainEngine:
 
         def view_q(i):
             return lambda t: t.view(Fr, Sp, 3, nh, dh)[:, :S, i]
-        for li in range(g.vit_layers):
+
+        def block(li, x):
             b = f"{v}blocks.{li}."
             self._mark([b + "attn.qkv.weight", b + "attn.out_proj.weight", b + "mlp.linear1.weight", b + "mlp.linear2.weight"])
             gw = (lambda n: self.gm(b + n)) if trv else (lambda n: None)
@@ -720,8 +760,10 @@ class TrainEngine:
             hpre = self.linear(y, self.w(b + "mlp.linear1.weight"), gw("mlp.linear1.weight"), self.v32(b + "mlp.linear1.bias"),
                                gb("mlp.linear1.bias"))
             hact = self.gelu(hpre)
-            x = self.linear(hact, self.w(b + "mlp.linear2.weight"), gw("mlp.linear2.weight"), self.v32(b + "mlp.linear2.bias"),
-                            gb("mlp.linear2.bias"), residual=x)
+            return self.linear(hact, self.w(b + "mlp.linear2.weight"), gw("mlp.linear2.weight"), self.v32(b + "mlp.linear2.bias"),
+                               gb("mlp.linear2.bias"), residual=x)
+        for li in range(g.vit_layers):
+            x = self._segment(functools.partial(block, li), x)
         y = self.layernorm(x, v + "norm.weight", v + "norm.bias", "vit")
         # drop cls + pooling
         npf = g.tokens_per_frame
@@ -896,9 +938,11 @@ class TrainEngine:
             del dpT
             for bi in range(B):
                 dsc = pT[bi]
-                if tr:  # dW_s += dsc [K, T] @ X_b [T, E]
+                if tr:  # dW_s (+)= dsc [K, T] @ X_b [T, E]: the step's first write overwrites the slot, like every wgrad
                     gws = self.gm(sname)
-                    ops.gemm(dsc, x3[bi], gws, M=K, N=E, K=Tn, lda=Tp, ldb=E, ldc=E, b_mn=True, residual=gws, ldr=E)
+                    acc = self._gm_begin_write(gws)
+                    ops.gemm(dsc, x3[bi], gws, M=K, N=E, K=Tn, lda=Tp, ldb=E, ldc=E, b_mn=True, residual=gws if acc else None,
+                             ldr=E if acc else 0)
                 if x.ng:  # dX_b += dsc^T [T, K] @ W_s [K, E]
                     ops.gemm(dsc, Ws, dx3[bi], M=Tn, N=E, K=K, lda=Tp, ldb=E, ldc=E, a_mn=True, b_mn=True, residual=dx3[bi], ldr=E)
             out.g = None
@@ -950,12 +994,15 @@ class TrainEngine:
         g = self.g
         E, Q = g.hidden_size, g.num_3d_query_token
         u = "model.u2tokenizer."
-        x = v_tokens
-        for i in range(g.u2t_num_layers):
+
+        def svr_layer(i, x):
             l = f"{u}svt_module.attention_network.layers.{i}."
             self._mark([k for k in self.lay.mat_names if k.startswith(l)])
             x = self._self_attention(x, B * C, N, l + "spatial_attention.")
-            x = self._temporal_attention(x, B, C, N, l + "temporal_attention.")
+            return self._temporal_attention(x, B, C, N, l + "temporal_attention.")
+        x = v_tokens
+        for i in range(g.u2t_num_layers):
+            x = self._segment(functools.partial(svr_layer, i), x)
         self._mark([u + "svt_module.token_selection.score_net.weight"])
         sel = self._token_selection_diff(x, B, C * N) if g.enable_diffts else self._token_selection_hard(x, B, C * N)
         if sel.v.dim() == 2:
@@ -978,7 +1025,8 @@ class TrainEngine:
         q = q_tok
         lin = u + "tta_module.layer_linagg.linear_aggregator."
         self._mark([lin + "wq.weight", lin + "wk.weight"])
-        for i in range(g.u2t_num_layers):
+
+        def tta_layer(i, q):
             l = f"{u}tta_module.layers_vt.{i}."
             self._mark([k for k in self.lay.mat_names if k.startswith(l)])
             s = self._self_attention(q, B, Q, l + "self_attention.")
@@ -986,7 +1034,9 @@ class TrainEngine:
             vx = self._cross_attention(s, vis, B, Q, Mv, l + "visual_cross_attention.", residual=None)
             vx = self.layernorm(vx, l + "norm_cross_v.weight", l + "norm_cross_v.bias", "u2t", residual=s)
             tx = self._cross_attention(vx, t_tokens, B, Q, Lt, l + "text_cross_attention.", residual=None)
-            q = self.layernorm(tx, l + "norm_cross_t.weight", l + "norm_cross_t.bias", "u2t", residual=vx)
+            return self.layernorm(tx, l + "norm_cross_t.weight", l + "norm_cross_t.bias", "u2t", residual=vx)
+        for i in range(g.u2t_num_layers):
+            q = self._segment(functools.partial(tta_layer, i), q)
         return self._cross_attention(q, vis, B, Q, Mv, u + "tta_module.layer_linagg.linear_aggregator.", residual=None, compress=True)
 
     # =========================================================================================
@@ -1035,7 +1085,8 @@ class TrainEngine:
         nh = hq + 2 * hkv
         tr = self._tr("dec")
         eps = g.rms_norm_eps
-        for li in range(g.num_hidden_layers):
+
+        def layer(li, x):
             l = f"model.layers.{li}."
             self._mark([k for k in self.lay.mat_names if k.startswith(l)])
             y = self.rmsnorm(x, l + "input_layernorm.weight", "dec", eps)
@@ -1052,7 +1103,9 @@ class TrainEngine:
             y = self.rmsnorm(x, l + "post_attention_layernorm.weight", "dec", eps)
             gu = self._dec_linear(y, li, 2, tr)
             act = self.silu_mul(gu)
-            x = self._dec_linear(act, li, 3, tr, residual=x)
+            return self._dec_linear(act, li, 3, tr, residual=x)
+        for li in range(g.num_hidden_layers):
+            x = self._segment(functools.partial(layer, li), x)
         return self.rmsnorm(x, "model.norm.weight", "dec", eps)
 
     def _dec_linear(self, x: Var, li: int, gi: int, tr: bool, residual: Optional[Var] = None) -> Var:
@@ -1223,6 +1276,7 @@ class TrainEngine:
         self.tape = []
         self.refresh_vectors()
         self._draw_lora_seed()
+        self._ckpt = bool(self.checkpoint)
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         lab = labels.to(self.dev, torch.int64)
         shift = torch.full_like(lab, -100)
@@ -1252,6 +1306,7 @@ class TrainEngine:
         self.tape = []
         self.refresh_vectors()
         self._lora_seed = 0
+        self._ckpt = False
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         lab = labels.to(self.dev, torch.int64)
         shift = torch.full_like(lab, -1)
@@ -1268,6 +1323,7 @@ class TrainEngine:
         self.tape = []
         self.refresh_vectors()
         self._lora_seed = 0
+        self._ckpt = False
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         labels, mask = _dpo_labels(input_ids.to(self.dev), loss_mask.to(self.dev))
         hname, Wh = self._head_w()
@@ -1282,6 +1338,7 @@ class TrainEngine:
         self.tape = []
         self.refresh_vectors()
         self._draw_lora_seed()
+        self._ckpt = bool(self.checkpoint)
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         labels, mask = _dpo_labels(input_ids.to(self.dev), loss_mask.to(self.dev))
         stats = {}
