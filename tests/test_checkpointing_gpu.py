@@ -37,14 +37,7 @@ def _weights(g, seed):
 
 def _grads(te):
     """{name: gradient} of every trainable parameter, cloned."""
-    L = te.lay
-    out = {}
-    for n in L.mat_names + L.vec_names:
-        if n in L.mat_off:
-            out[n] = te.Gm[L.mat_off[n]:L.mat_off[n] + L._numel(n)].view(L.shapes[n]).clone()
-        else:
-            out[n] = te.Gv[L.vec_off[n]:L.vec_off[n] + L._numel(n)].view(L.shapes[n]).clone()
-    return out
+    return {n: te.grad(n).clone() for n in te.lay.mat_names + te.lay.vec_names}
 
 
 def _check_oracle(te, ref_g):

@@ -336,8 +336,7 @@ def _compare_grads(te, ref_g, skip=()):
     for n in L.mat_names + L.vec_names:
         if n in skip or (n == "lm_head.weight" and te.tied):
             continue
-        got = (te.Gm[L.mat_off[n]:L.mat_off[n] + L._numel(n)] if n in L.mat_off else
-               te.Gv[L.vec_off[n]:L.vec_off[n] + L._numel(n)]).view(L.shapes[n]).float().cpu()
+        got = te.grad(n).float().cpu()
         want = ref_g[n].cpu()
         if want.abs().max().item() < 1e-9:
             continue

@@ -443,10 +443,7 @@ def test_forward_backward_matches_oracle_autograd(case):
     # tensor also passes when its absolute error is below 2e-3 of the largest gradient entry of the whole model
     gmax = max(v.abs().max().item() for v in ref_g.values())
     for n in L.mat_names + L.vec_names:
-        if n in L.mat_off:
-            got = te.Gm[L.mat_off[n]:L.mat_off[n] + L._numel(n)].view(L.shapes[n]).float().cpu()
-        else:
-            got = te.Gv[L.vec_off[n]:L.vec_off[n] + L._numel(n)].view(L.shapes[n]).float().cpu()
+        got = te.grad(n).float().cpu()
         if n == "lm_head.weight" and te.tied:
             continue
         want = ref_g[n].cpu()
@@ -566,17 +563,14 @@ def test_gradient_slots_overwrite_accumulate_and_stale_clear():
     assert err <= 2e-2 * want.abs().max().item() + 1e-6, err
     close(te.Gv, gva + fresh.Gv, 1e-3, "accumulated vector gradients")
     # a group that stops training: its slots are cleared when the step does not write them
-    L = te.lay
     vit_w = "model.vision_tower.vision_tower.blocks.0.mlp.linear1.weight"
-    sl = slice(L.mat_off[vit_w], L.mat_off[vit_w] + L._numel(vit_w))
-    assert te.Gm[sl].abs().max().item() > 0
+    assert te.grad(vit_w).abs().max().item() > 0
     te.trainable["vit"] = False
     te.zero_grad()
     run(te, ib, idb, qb, lb)
-    assert te.Gm[sl].abs().max().item() == 0
+    assert te.grad(vit_w).abs().max().item() == 0
     dec_w = "model.layers.0.mlp.down_proj.weight"
-    sd_ = slice(L.mat_off[dec_w], L.mat_off[dec_w] + L._numel(dec_w))
-    assert (te.Gm[sd_].float() - fresh.Gm[sd_].float()).abs().max().item() <= 4e-3 * gmax
+    assert (te.grad(dec_w).float() - fresh.grad(dec_w).float()).abs().max().item() <= 4e-3 * gmax
 
 
 def test_module_backward_accumulates_over_micro_batches():
@@ -698,8 +692,7 @@ def test_dpo_step_matches_oracle_autograd():
         want = sd[n].grad
         if want is None or want.abs().max().item() < 1e-9:
             continue
-        got = (te.Gm[L.mat_off[n]:L.mat_off[n] + L._numel(n)] if n in L.mat_off else te.Gv[L.vec_off[n]:L.vec_off[n] + L._numel(n)])
-        got = got.view(L.shapes[n]).float().cpu()
+        got = te.grad(n).float().cpu()
         want = want.cpu()
         e, c = rel_err(got, want), cosine(got, want)
         if not (e < 4e-2 and c > 0.995) and (got - want).abs().max().item() >= 2e-3 * gmax:

@@ -26,10 +26,7 @@ torch.cuda.synchronize()
 print("loss", float(loss), ref_loss)
 L = te.lay
 for n in L.mat_names + L.vec_names:
-    if n in L.mat_off:
-        got = te.Gm[L.mat_off[n]:L.mat_off[n] + L._numel(n)].view(L.shapes[n]).float().cpu()
-    else:
-        got = te.Gv[L.vec_off[n]:L.vec_off[n] + L._numel(n)].view(L.shapes[n]).float().cpu()
+    got = te.grad(n).float().cpu()
     want = ref_g.get(n)
     if want is None:
         continue

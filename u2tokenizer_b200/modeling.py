@@ -630,31 +630,13 @@ class _U2TrainLoss(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out):
         te = ctx.te
-        L = te.lay
         # autograd keeps the returned views as p.grad (no copy): on the next micro-batch of a gradient-accumulation window
         # those p.grad ARE the matrix slots, so the kernels add into them in place and nothing is handed back for them
-        def slot(n):
-            return te.Gm[L.mat_off[n]:L.mat_off[n] + L._numel(n)]
         keep = {n for n, p in zip(ctx.names, ctx.params)
-                if n in L.mat_off and p.grad is not None and p.grad.data_ptr() == slot(n).data_ptr()}
+                if n in te.lay.mat_off and p.grad is not None and p.grad.data_ptr() == te.grad(n).data_ptr()}
         te.zero_grad(keep=keep)
         te.backward(grad_out.to(torch.float32))
-        gvb = torch.empty(L.vec_total, device=te.dev, dtype=torch.bfloat16)
-        from . import train_ops as T
-        T.cast(te.Gv, gvb)
-        grads = []
-        for n in ctx.names:
-            if n == "lm_head.weight" and te.tied:
-                grads.append(None)   # the tied head's gradient is delivered through embed_tokens
-            elif n in keep:
-                grads.append(None)   # already accumulated in place
-            elif n in L.mat_off:
-                grads.append(slot(n).view(L.shapes[n]))
-            elif n in L.vec_off:
-                grads.append(gvb[L.vec_off[n]:L.vec_off[n] + L._numel(n)].view(L.shapes[n]))
-            else:
-                grads.append(None)
-        return (None, None, None, *grads)
+        return (None, None, None, *te.param_grads(ctx.names, keep))
 
 
 # ------------------------------------------------------------------------------------------------

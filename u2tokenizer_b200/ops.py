@@ -21,7 +21,9 @@ DT_BF16, DT_F32 = 0, 1
 
 
 def _stream() -> int:
-    return torch.cuda.current_stream().cuda_stream
+    # the device index is passed explicitly: without it torch.cuda.current_stream() re-resolves the current device
+    # through its availability checks on every call, host time that the launch-bound training forward pays per kernel
+    return torch.cuda.current_stream(torch.cuda.current_device()).cuda_stream
 
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:

@@ -174,6 +174,8 @@ class Layout:
         return k
 
     def adjacent(self, names: Sequence[str]) -> bool:
+        if len(names) == 1:
+            return True
         tab = next(t for t in (self.mat_off, self.vec_off, self.frozen_off) if names[0] in t)
         for a, b in zip(names[:-1], names[1:]):
             if tab[a] + self._numel(a) != tab[b]:
@@ -314,6 +316,33 @@ class TrainEngine:
         off = L.vec_off[names[0]]
         return self.Gv[off:off + sum(L._numel(n) for n in names)]
 
+    def grad(self, n: str) -> torch.Tensor:
+        """Gradient of parameter n in its parameter shape: a view of its bf16 slot in Gm (matrices) or its fp32 slot in Gv
+        (vectors)."""
+        L = self.lay
+        buf, off = (self.Gm, L.mat_off[n]) if n in L.mat_off else (self.Gv, L.vec_off[n])
+        return buf[off:off + L._numel(n)].view(L.shapes[n])
+
+    def param_grads(self, names: Sequence[str], keep=()) -> List[Optional[torch.Tensor]]:
+        """The gradients autograd hands to the module parameters `names` after backward(): matrices get their Gm slot (no
+        copy), vectors a view of one bf16 cast of Gv. None for the tied lm_head (its gradient is delivered through
+        embed_tokens), for names in `keep` (their p.grad already is the slot, accumulated in place) and for parameters
+        without a slot (frozen)."""
+        L = self.lay
+        gvb = torch.empty(L.vec_total, device=self.dev, dtype=BF16)
+        T.cast(self.Gv, gvb)
+        out = []
+        for n in names:
+            if (n == "lm_head.weight" and self.tied) or n in keep:
+                out.append(None)
+            elif n in L.mat_off:
+                out.append(self.grad(n))
+            elif n in L.vec_off:
+                out.append(gvb[L.vec_off[n]:L.vec_off[n] + L._numel(n)].view(L.shapes[n]))
+            else:
+                out.append(None)
+        return out
+
     def refresh_vectors(self):
         """fp32 mirrors of the vector parameters (biases, norm weights, bias tables) from their bf16 values."""
         L = self.lay
@@ -321,7 +350,7 @@ class TrainEngine:
 
     def bind_module(self, model) -> None:
         """Re-point the module's nn.Parameters at the flat buffer (no second copy of the weights); gradients are
-        exposed the same way after backward (see grads_for_module)."""
+        exposed the same way after backward (see param_grads)."""
         sd_names = dict(model.named_parameters())
         for n, p in sd_names.items():
             n = n.replace(".base_layer.", ".")   # a LoRA target's base weight (PEFT module layout)
@@ -404,6 +433,27 @@ class TrainEngine:
         else:
             T.add_(var.g, t.view(var.g.shape) if t.is_contiguous() else t.contiguous().view(var.g.shape))
 
+    def _backward(self, out: Var, fn):
+        """Tape entry of the op that produced `out`: the backward calls fn(out.g) (see _run_tape)."""
+        self.tape.append((out, fn))
+
+    def _run_tape(self, tape):
+        """Run a tape in reverse. An op's entry (out, fn) runs fn(out.g) only when out received a gradient, and releases
+        that gradient right after (a checkpointed segment's recompute relies on every op freeing its output's gradient);
+        an entry without an output (marker, segment recompute, loss head) always runs."""
+        for out, fn in reversed(tape):
+            if out is None:
+                fn()
+            elif out.g is not None:
+                fn(out.g)
+                out.g = None
+
+    def _reshape(self, var: Var, shape) -> Var:
+        """A Var over a reshaped view of var.v; its gradient is routed back to var."""
+        out = Var(var.v.view(shape), var.ng)
+        self._backward(out, lambda dy: self._acc(var, dy.view(var.v.shape), owned=True))
+        return out
+
     def _tr(self, group: str) -> bool:
         return bool(self.trainable.get(group, True))
 
@@ -444,7 +494,7 @@ class TrainEngine:
                         with torch.cuda.stream(self.comm_stream):
                             self.comm_stream.wait_event(ev)
                             self.reduce_bucket(b)
-        self.tape.append(done)
+        self.tape.append((None, done))
 
     def _segment(self, body, x: Var) -> Var:
         """One repeated block (ViT block, SVR layer, TTA layer, decoder layer): out = body(x), body starting with the
@@ -472,9 +522,8 @@ class TrainEngine:
             finally:
                 self.tape, self._lora_seed = outer_, seed_
             out2.g, out.g = out.g, None
-            for fn in reversed(local):
-                fn()
-        self.tape.append(bwd)
+            self._run_tape(local)
+        self.tape.append((None, bwd))
         return out
 
     # ---- linear ---------------------------------------------------------------------------------
@@ -484,10 +533,7 @@ class TrainEngine:
         y = ops.linear(x.v, w, bias, residual=residual.v if residual is not None else None)
         out = Var(y, x.ng or gw is not None or (residual is not None and residual.ng))
 
-        def bwd():
-            dy = out.g
-            if dy is None:
-                return
+        def bwd(dy):
             if gw is not None:
                 self.wgrad(dy, x.v, gw)
             if gbias is not None:
@@ -499,9 +545,18 @@ class TrainEngine:
                     T.linear_dgrad(dy, w, out=x.g, accumulate=True)
             if residual is not None:
                 self._acc(residual, dy, owned=True)
-            out.g = None
-        self.tape.append(bwd)
+        self._backward(out, bwd)
         return out
+
+    def _param_linear(self, x: Var, weights, biases, group: str, residual: Optional[Var] = None) -> Var:
+        """linear() on named parameters: weights / biases one name or a list of adjacent names (one fused GEMM: q|k|v,
+        wk|wv, gate|up), biases may be None. Gradient slots only while `group` trains."""
+        ws = [weights] if isinstance(weights, str) else weights
+        bs = [biases] if isinstance(biases, str) else biases
+        gw = gb = None
+        if self._tr(group):
+            gw, gb = self.gm(ws), (self.gv(bs) if bs else None)
+        return self.linear(x, self.wcat(ws), gw, self.v32cat(bs) if bs else None, gb, residual=residual)
 
     # ---- norms ------------------------------------------------------------------------------------
     def layernorm(self, x: Var, gname: str, bname: str, group: str, eps: float = 1e-5, residual: Optional[Var] = None) -> Var:
@@ -514,62 +569,52 @@ class TrainEngine:
             s = x.v
             y = ops.layernorm(x.v, gamma, beta, eps)
         out = Var(y, True)
-        tr = self._tr(group)
+        dgamma, dbeta = (self.gv(gname), self.gv(bname)) if self._tr(group) else (None, None)
 
-        def bwd():
-            if out.g is None:
-                return
-            need_dx = x.ng or (residual is not None and residual.ng)
-            if need_dx or tr:
+        def bwd(dy):
+            if x.ng or (residual is not None and residual.ng) or dgamma is not None:
                 pend = x.g if (x.g is not None and residual is None) else None
-                dx = T.layernorm_bwd(s, gamma, out.g, dres=pend, out=pend, dgamma=self.gv(gname) if tr else None,
-                                     dbeta=self.gv(bname) if tr else None, eps=eps)
+                dx = T.layernorm_bwd(s, gamma, dy, dres=pend, out=pend, dgamma=dgamma, dbeta=dbeta, eps=eps)
                 if pend is None:
                     if residual is not None:
                         self._acc(x, dx, owned=False)
                         self._acc(residual, dx, owned=True)
                     else:
                         self._acc(x, dx, owned=True)
-            out.g = None
-        self.tape.append(bwd)
+        self._backward(out, bwd)
         return out
 
     def rmsnorm(self, x: Var, gname: str, group: str, eps: float) -> Var:
         gamma = self.v32(gname)
         y = ops.rmsnorm(x.v, gamma, eps)
         out = Var(y, True)
-        tr = self._tr(group)
+        dgamma = self.gv(gname) if self._tr(group) else None
 
-        def bwd():
-            if out.g is None:
-                return
+        def bwd(dy):
             pend = x.g
-            dx = T.rmsnorm_bwd(x.v, gamma, out.g, dres=pend, out=pend, dgamma=self.gv(gname) if tr else None, eps=eps)
+            dx = T.rmsnorm_bwd(x.v, gamma, dy, dres=pend, out=pend, dgamma=dgamma, eps=eps)
             if pend is None:
                 self._acc(x, dx, owned=True)
-            out.g = None
-        self.tape.append(bwd)
+        self._backward(out, bwd)
         return out
 
     # ---- activations --------------------------------------------------------------------------------
     def gelu(self, x: Var) -> Var:
         out = Var(T.gelu(x.v), x.ng)
 
-        def bwd():
-            if out.g is not None and x.ng:
-                self._acc(x, T.gelu_bwd(x.v, out.g), owned=True)
-            out.g = None
-        self.tape.append(bwd)
+        def bwd(dy):
+            if x.ng:
+                self._acc(x, T.gelu_bwd(x.v, dy), owned=True)
+        self._backward(out, bwd)
         return out
 
     def silu_mul(self, gu: Var) -> Var:
         out = Var(ops.silu_mul(gu.v, interleaved=False), gu.ng)
 
-        def bwd():
-            if out.g is not None and gu.ng:
-                self._acc(gu, T.silu_mul_bwd(gu.v, out.g), owned=True)
-            out.g = None
-        self.tape.append(bwd)
+        def bwd(dy):
+            if gu.ng:
+                self._acc(gu, T.silu_mul_bwd(gu.v, dy), owned=True)
+        self._backward(out, bwd)
         return out
 
     # ---- attention through the GEMM (scores fp32, probabilities bf16 kept for the backward) -----------
@@ -617,10 +662,8 @@ class TrainEngine:
         out = Var(ctx_full, qv.ng or kv.ng or vv.ng)
         tr_rel = rel_name is not None and self._tr(group)
 
-        def bwd():
-            if out.g is None:
-                return
-            do = out.g[:, :Sq].view(b, Sq, h, dh)
+        def bwd(dy):
+            do = dy[:, :Sq].view(b, Sq, h, dh)
             pr = saved.pop("p", None)
             lse = saved.pop("lse", None)
             if pr is None and lse is not None:
@@ -674,8 +717,7 @@ class TrainEngine:
             if kv.ng:
                 dk = k_view(kv.g)
                 self._pt_gemm(pr, q, dk, b, h, hk, Sq, Sk, Skp, dh, scale, accumulate=not fresh[id(kv)])
-            out.g = None
-        self.tape.append(bwd)
+        self._backward(out, bwd)
         return out
 
     def _pt_gemm(self, p: torch.Tensor, x: torch.Tensor, dst: torch.Tensor, b, h, hk, Sq, Sk, Skp, dh, alpha, accumulate):
@@ -719,21 +761,19 @@ class TrainEngine:
         ops.gemm(rows, pe_w, x0, M=Fr * P, N=Hd, K=g.patch_dim, lda=g.patch_dim, ldb=g.patch_dim, ldc=Hd, bias=pe_b,
                  residual=pos, ldr=Hd, res_row_mod=P, row_remap=(P, Sp, 1))
         ops.vit_frame_rows(x0, self.w(v + "cls_token").view(Hd), Fr, Sp, S)
-        x_emb = Var(x0.view(Fr * Sp, Hd), trv)   # NOT `x`: that name is rebound by the layer loop below
+        x = Var(x0.view(Fr * Sp, Hd), trv)
         self._mark([v + "patch_embedding.patch_embeddings.1.weight"])
 
-        def bwd_embed():
-            if x_emb.g is None or not trv:
+        def bwd_embed(dx):
+            if not trv:
                 return
-            dx = x_emb.g.view(Fr, Sp, Hd)
+            dx = dx.view(Fr, Sp, Hd)
             dy = dx[:, 1:1 + P].contiguous().view(Fr * P, Hd)
             self.wgrad(dy, rows, self.gm(v + "patch_embedding.patch_embeddings.1.weight"))
             T.colsum(dy, self.gv(v + "patch_embedding.patch_embeddings.1.bias"))
             T.colsum(dy, self.gv(v + "patch_embedding.position_embeddings"), rows=Fr, cols=P * Hd, ld=P * Hd)
             T.colsum(dx, self.gv(v + "cls_token"), rows=Fr, cols=Hd, ld=Sp * Hd)
-            x_emb.g = None
-        self.tape.append(bwd_embed)
-        x = x_emb
+        self._backward(x, bwd_embed)
 
         nh = g.vit_heads
         dh = Hd // nh
@@ -744,24 +784,16 @@ class TrainEngine:
         def block(li, x):
             b = f"{v}blocks.{li}."
             self._mark([b + "attn.qkv.weight", b + "attn.out_proj.weight", b + "mlp.linear1.weight", b + "mlp.linear2.weight"])
-            gw = (lambda n: self.gm(b + n)) if trv else (lambda n: None)
-            gb = (lambda n: self.gv(b + n)) if trv else (lambda n: None)
             y = self.layernorm(x, b + "norm1.weight", b + "norm1.bias", "vit")
-            has_qb = (b + "attn.qkv.bias") in self.lay.shapes
-            qkv = self.linear(y, self.w(b + "attn.qkv.weight"), gw("attn.qkv.weight"),
-                              self.v32(b + "attn.qkv.bias") if has_qb else None, gb("attn.qkv.bias") if has_qb else None)
+            qb = b + "attn.qkv.bias"
+            qkv = self._param_linear(y, b + "attn.qkv.weight", qb if qb in self.lay.shapes else None, "vit")
             ctx = self.attention(qkv, view_q(0), qkv, view_q(1), qkv, view_q(2), (Fr, Sp, Hd), dh ** -0.5, group="vit",
                                  recompute=True)
-            ctx2 = Var(ctx.v.view(Fr * Sp, Hd), ctx.ng)
-            self._alias(ctx2, ctx)
-            x = self.linear(ctx2, self.w(b + "attn.out_proj.weight"), gw("attn.out_proj.weight"), self.v32(b + "attn.out_proj.bias"),
-                            gb("attn.out_proj.bias"), residual=x)
+            ctx = self._reshape(ctx, (Fr * Sp, Hd))
+            x = self._param_linear(ctx, b + "attn.out_proj.weight", b + "attn.out_proj.bias", "vit", residual=x)
             y = self.layernorm(x, b + "norm2.weight", b + "norm2.bias", "vit")
-            hpre = self.linear(y, self.w(b + "mlp.linear1.weight"), gw("mlp.linear1.weight"), self.v32(b + "mlp.linear1.bias"),
-                               gb("mlp.linear1.bias"))
-            hact = self.gelu(hpre)
-            return self.linear(hact, self.w(b + "mlp.linear2.weight"), gw("mlp.linear2.weight"), self.v32(b + "mlp.linear2.bias"),
-                               gb("mlp.linear2.bias"), residual=x)
+            h = self.gelu(self._param_linear(y, b + "mlp.linear1.weight", b + "mlp.linear1.bias", "vit"))
+            return self._param_linear(h, b + "mlp.linear2.weight", b + "mlp.linear2.bias", "vit", residual=x)
         for li in range(g.vit_layers):
             x = self._segment(functools.partial(block, li), x)
         y = self.layernorm(x, v + "norm.weight", v + "norm.bias", "vit")
@@ -771,63 +803,44 @@ class TrainEngine:
         seq = g.proj_pooling_type == "sequence"
         ops.spp_pool(y.v, pooled, frames=Fr, grid=g.grid, ps=g.proj_pooling_size, E=Hd, in_frame_stride=Sp, in_off=1, ldx=Hd,
                      sequence=seq)
-        z_pool = Var(pooled.view(Fr * npf, Hd), y.ng)   # `z` is rebound by the projector loop
-        y_ln = y
+        z = Var(pooled.view(Fr * npf, Hd), y.ng)
 
-        def bwd_pool():
-            if z_pool.g is None or not y_ln.ng:
+        def bwd_pool(dz):
+            if not y.ng:
                 return
             dy = torch.empty(Fr * Sp, Hd, device=self.dev, dtype=BF16)
-            T.spp_pool_bwd(z_pool.g, dy, frames=Fr, grid=g.grid, ps=g.proj_pooling_size, E=Hd, in_frame_stride=Sp, in_off=1, ldx=Hd,
+            T.spp_pool_bwd(dz, dy, frames=Fr, grid=g.grid, ps=g.proj_pooling_size, E=Hd, in_frame_stride=Sp, in_off=1, ldx=Hd,
                            rows_per_frame=Sp, sequence=seq)
-            self._acc(y_ln, dy, owned=True)
-            z_pool.g = None
-        self.tape.append(bwd_pool)
-        z = z_pool
+            self._acc(y, dy, owned=True)
+        self._backward(z, bwd_pool)
         # projector MLP
-        trp = self._tr("proj")
         p = "model.mm_projector.projector."
         n = int(g.proj_layer_num)
         self._mark([k for k in self.lay.mat_names if k.startswith(p)])
         for i in range(n):
             idx = (2 * i if g.proj_layer_type == "mlp" else i) if i else 0
-            z = self.linear(z, self.w(p + f"{idx}.weight"), self.gm(p + f"{idx}.weight") if trp else None,
-                            self.v32(p + f"{idx}.bias"), self.gv(p + f"{idx}.bias") if trp else None)
+            z = self._param_linear(z, p + f"{idx}.weight", p + f"{idx}.bias", "proj")
             if g.proj_layer_type == "mlp" and i < n - 1:
                 z = self.gelu(z)
         return z
 
-    def _alias(self, view_var: Var, base: Var):
-        """view_var.v is a reshaped view of base.v: route its gradient to base."""
-        def bwd():
-            if view_var.g is not None:
-                self._acc(base, view_var.g.view(base.v.shape), owned=True)
-                view_var.g = None
-        self.tape.append(bwd)
-
     # =========================================================================================
     # mu2-tokenizer
     # =========================================================================================
-    def _attn_names(self, pre: str):
-        return ([pre + "wq.weight", pre + "wk.weight", pre + "wv.weight"], [pre + "wq.bias", pre + "wk.bias", pre + "wv.bias"])
-
     def _self_attention(self, x: Var, nb: int, S: int, pre: str, residual: Optional[Var] = None) -> Var:
         """RMA / RoPE self attention over nb sequences of length S (reference rma.py:46-82, rope.py:62-91)."""
         g = self.g
         E, H = g.hidden_size, g.u2t_num_heads
         dh = E // H
-        tr = self._tr("u2t")
-        wn, bn = self._attn_names(pre)
-        qkv = self.linear(x, self.wcat(wn), self.gm(wn) if tr else None, self.v32cat(bn), self.gv(bn) if tr else None)
+        qkv = self._param_linear(x, [pre + "wq.weight", pre + "wk.weight", pre + "wv.weight"],
+                                 [pre + "wq.bias", pre + "wk.bias", pre + "wv.bias"], "u2t")
         if g.attn_type == "rope":
             qkv = self._rope_tok(qkv, rows=nb * S, pos_div=1, pos_mod=S)
         view = lambda i: (lambda t: t.view(nb, S, 3, H, dh)[:, :, i])
         ctx = self.attention(qkv, view(0), qkv, view(1), qkv, view(2), (nb, S, E), 1.0 / math.sqrt(dh),
                              rel_name=(pre + "relative_bias") if g.attn_type == "rma" else None)
-        c2 = Var(ctx.v.view(nb * S, E), ctx.ng)
-        self._alias(c2, ctx)
-        return self.linear(c2, self.w(pre + "dense.weight"), self.gm(pre + "dense.weight") if tr else None,
-                           self.v32(pre + "dense.bias"), self.gv(pre + "dense.bias") if tr else None, residual=residual)
+        return self._param_linear(self._reshape(ctx, (nb * S, E)), pre + "dense.weight", pre + "dense.bias", "u2t",
+                                  residual=residual)
 
     def _rope_tok(self, qkv: Var, rows: int, pos_div: int, pos_mod: int) -> Var:
         g = self.g
@@ -837,22 +850,20 @@ class TrainEngine:
         ops.rope(y, rows=rows, ld=3 * E, dh=dh, n_q=H, n_k=H, inv_freq=self.u2t_inv_freq, pos_div=pos_div, pos_mod=pos_mod)
         out = Var(y, qkv.ng)
 
-        def bwd():
-            if out.g is not None and qkv.ng:
-                T.rope_bwd(out.g, None, rows=rows, ld=3 * E, dh=dh, n_q=H, n_k=H, inv_freq=self.u2t_inv_freq, pos_div=pos_div,
+        def bwd(dy):
+            if qkv.ng:
+                T.rope_bwd(dy, None, rows=rows, ld=3 * E, dh=dh, n_q=H, n_k=H, inv_freq=self.u2t_inv_freq, pos_div=pos_div,
                            pos_mod=pos_mod)
-                self._acc(qkv, out.g, owned=True)
-            out.g = None
-        self.tape.append(bwd)
+                self._acc(qkv, dy, owned=True)
+        self._backward(out, bwd)
         return out
 
     def _temporal_attention(self, x: Var, B: int, C: int, N: int, pre: str) -> Var:
         g = self.g
         E, H = g.hidden_size, g.u2t_num_heads
         dh = E // H
-        tr = self._tr("u2t")
-        wn, bn = self._attn_names(pre)
-        qkv = self.linear(x, self.wcat(wn), self.gm(wn) if tr else None, self.v32cat(bn), self.gv(bn) if tr else None)
+        qkv = self._param_linear(x, [pre + "wq.weight", pre + "wk.weight", pre + "wv.weight"],
+                                 [pre + "wq.bias", pre + "wk.bias", pre + "wv.bias"], "u2t")
         if g.attn_type == "rope":
             qkv = self._rope_tok(qkv, rows=B * C * N, pos_div=N, pos_mod=C)
         rel = self.v32(pre + "relative_bias").view(-1) if g.attn_type == "rma" else None
@@ -860,17 +871,16 @@ class TrainEngine:
         ctxv = torch.empty(B * C * N, E, device=self.dev, dtype=BF16)
         ops.temporal_attention(qkv.v, ctxv, B=B, C_=C, N=N, H=H, dh=dh, scale=scale, rel_bias=rel, rel_max=REL_MAX)
         ctx = Var(ctxv, qkv.ng)
+        drel = self.gv(pre + "relative_bias") if (rel is not None and self._tr("u2t")) else None
 
-        def bwd():
-            if ctx.g is not None and qkv.ng:
+        def bwd(dctx):
+            if qkv.ng:
                 dqkv = torch.empty_like(qkv.v)
-                T.temporal_attention_bwd(qkv.v, ctx.g, dqkv, B=B, C_=C, N=N, H=H, dh=dh, scale=scale, rel_bias=rel,
-                                         drel=self.gv(pre + "relative_bias") if (rel is not None and tr) else None, rel_max=REL_MAX)
+                T.temporal_attention_bwd(qkv.v, dctx, dqkv, B=B, C_=C, N=N, H=H, dh=dh, scale=scale, rel_bias=rel, drel=drel,
+                                         rel_max=REL_MAX)
                 self._acc(qkv, dqkv, owned=True)
-            ctx.g = None
-        self.tape.append(bwd)
-        return self.linear(ctx, self.w(pre + "dense.weight"), self.gm(pre + "dense.weight") if tr else None,
-                           self.v32(pre + "dense.bias"), self.gv(pre + "dense.bias") if tr else None)
+        self._backward(ctx, bwd)
+        return self._param_linear(ctx, pre + "dense.weight", pre + "dense.bias", "u2t")
 
     def _cross_attention(self, q_in: Var, kv_in: Var, B: int, Sq: int, Sk: int, pre: str, residual: Optional[Var],
                          compress: bool = False) -> Var:
@@ -878,26 +888,18 @@ class TrainEngine:
         g = self.g
         E, H = g.hidden_size, g.u2t_num_heads
         dh = E // H
-        tr = self._tr("u2t")
-        q = self.linear(q_in, self.w(pre + "wq.weight"), self.gm(pre + "wq.weight") if tr else None, self.v32(pre + "wq.bias"),
-                        self.gv(pre + "wq.bias") if tr else None)
+        q = self._param_linear(q_in, pre + "wq.weight", pre + "wq.bias", "u2t")
         qview = lambda t: t.view(B, Sq, H, dh)
         if compress:
-            k = self.linear(kv_in, self.w(pre + "wk.weight"), self.gm(pre + "wk.weight") if tr else None,
-                            self.v32(pre + "wk.bias"), self.gv(pre + "wk.bias") if tr else None)
+            k = self._param_linear(kv_in, pre + "wk.weight", pre + "wk.bias", "u2t")
             kview = lambda t: t.view(B, Sk, H, dh)
             ctx = self.attention(q, qview, k, kview, kv_in, kview, (B, Sq, E), 1.0 / math.sqrt(dh))
-            c2 = Var(ctx.v.view(B * Sq, E), ctx.ng)
-            self._alias(c2, ctx)
-            return c2
-        wn, bn = [pre + "wk.weight", pre + "wv.weight"], [pre + "wk.bias", pre + "wv.bias"]
-        kvp = self.linear(kv_in, self.wcat(wn), self.gm(wn) if tr else None, self.v32cat(bn), self.gv(bn) if tr else None)
+            return self._reshape(ctx, (B * Sq, E))
+        kvp = self._param_linear(kv_in, [pre + "wk.weight", pre + "wv.weight"], [pre + "wk.bias", pre + "wv.bias"], "u2t")
         kview = lambda i: (lambda t: t.view(B, Sk, 2, H, dh)[:, :, i])
         ctx = self.attention(q, qview, kvp, kview(0), kvp, kview(1), (B, Sq, E), 1.0 / math.sqrt(dh))
-        c2 = Var(ctx.v.view(B * Sq, E), ctx.ng)
-        self._alias(c2, ctx)
-        return self.linear(c2, self.w(pre + "dense.weight"), self.gm(pre + "dense.weight") if tr else None,
-                           self.v32(pre + "dense.bias"), self.gv(pre + "dense.bias") if tr else None, residual=residual)
+        return self._param_linear(self._reshape(ctx, (B * Sq, E)), pre + "dense.weight", pre + "dense.bias", "u2t",
+                                  residual=residual)
 
     def _token_selection_diff(self, x: Var, B: int, Tn: int) -> Var:
         """DifferentiableTokenSelection (reference svr.py:101-117): softmax over the TOKEN axis of W_s X^T, selected =
@@ -920,10 +922,7 @@ class TrainEngine:
                  c_strides=(0, K * E), b_mn=True)
         out = Var(sel, x.ng or tr)
 
-        def bwd():
-            if out.g is None:
-                return
-            ds = out.g
+        def bwd(ds):
             if x.ng and x.g is None:
                 x.g = torch.zeros_like(x.v)
             dx3 = x.g.view(B, Tn, E) if x.ng else None
@@ -945,8 +944,7 @@ class TrainEngine:
                              ldr=E if acc else 0)
                 if x.ng:  # dX_b += dsc^T [T, K] @ W_s [K, E]
                     ops.gemm(dsc, Ws, dx3[bi], M=Tn, N=E, K=K, lda=Tp, ldb=E, ldc=E, a_mn=True, b_mn=True, residual=dx3[bi], ldr=E)
-            out.g = None
-        self.tape.append(bwd)
+        self._backward(out, bwd)
         return out
 
     def _token_selection_hard(self, x: Var, B: int, Tn: int) -> Var:
@@ -962,13 +960,12 @@ class TrainEngine:
         idx = ops.topk_rows(sc.view(B, Tn), K, idx_offset_per_row=Tn)
         out = Var(ops.embed_splice(idx, x.v, None), x.ng)
 
-        def bwd():
-            if out.g is not None and x.ng:
+        def bwd(dy):
+            if x.ng:
                 if x.g is None:
                     x.g = torch.zeros_like(x.v)
-                T.embed_scatter_add(idx, out.g, x.g, None)
-            out.g = None
-        self.tape.append(bwd)
+                T.embed_scatter_add(idx, dy, x.g, None)
+        self._backward(out, bwd)
         return out
 
     def _multiscale(self, x: Var, B: int) -> Var:
@@ -978,15 +975,12 @@ class TrainEngine:
         K, E = x.v.shape[1], x.v.shape[2]
         y, logits = T.multiscale_pool_fwd(x.v, gate_w, g.enable_dmtp)
         out = Var(y, x.ng)
-        tr = self._tr("u2t")
+        dgate = self.gv(gname) if (g.enable_dmtp and self._tr("u2t")) else None
 
-        def bwd():
-            if out.g is not None and x.ng:
-                dx = T.multiscale_pool_bwd(x.v, out.g, gate_w, logits, self.gv(gname) if (g.enable_dmtp and tr) else None,
-                                           g.enable_dmtp)
-                self._acc(x, dx, owned=True)
-            out.g = None
-        self.tape.append(bwd)
+        def bwd(dy):
+            if x.ng:
+                self._acc(x, T.multiscale_pool_bwd(x.v, dy, gate_w, logits, dgate, g.enable_dmtp), owned=True)
+        self._backward(out, bwd)
         return out
 
     def u2tokenizer(self, v_tokens: Var, B: int, C: int, N: int, t_tokens: Var, Lt: int) -> Var:
@@ -1006,23 +1000,18 @@ class TrainEngine:
         self._mark([u + "svt_module.token_selection.score_net.weight"])
         sel = self._token_selection_diff(x, B, C * N) if g.enable_diffts else self._token_selection_hard(x, B, C * N)
         if sel.v.dim() == 2:
-            s3 = Var(sel.v.view(B, -1, E), sel.ng)
-            self._alias(s3, sel)
-            sel = s3
+            sel = self._reshape(sel, (B, -1, E))
         vis3 = self._multiscale(sel, B) if g.use_multi_scale else sel
         Mv = vis3.v.shape[1]
-        vis = Var(vis3.v.view(B * Mv, E), vis3.ng)
-        self._alias(vis, vis3)
+        vis = self._reshape(vis3, (B * Mv, E))
         tr = self._tr("u2t")
         qtok = self.w(u + "query_tokens").view(Q, E)
-        q_tok = Var(qtok.unsqueeze(0).expand(B, Q, E).contiguous().view(B * Q, E), tr)   # `q` is rebound per TTA layer
+        q = Var(qtok.unsqueeze(0).expand(B, Q, E).contiguous().view(B * Q, E), tr)
 
-        def bwd_q():
-            if q_tok.g is not None and tr:
-                T.colsum(q_tok.g, self.gv(u + "query_tokens"), rows=B, cols=Q * E, ld=Q * E)
-            q_tok.g = None
-        self.tape.append(bwd_q)
-        q = q_tok
+        def bwd_q(dq):
+            if tr:
+                T.colsum(dq, self.gv(u + "query_tokens"), rows=B, cols=Q * E, ld=Q * E)
+        self._backward(q, bwd_q)
         lin = u + "tta_module.layer_linagg.linear_aggregator."
         self._mark([lin + "wq.weight", lin + "wk.weight"])
 
@@ -1048,11 +1037,10 @@ class TrainEngine:
         B, Lx = ids.shape
         out = Var(ops.embed_splice(ids, table, None).view(B * Lx, -1), self._tr("embed"))
 
-        def bwd():
-            if out.g is not None and self._tr("embed"):
-                T.embed_scatter_add(ids, out.g.contiguous(), self._gm_scatter_target("model.embed_tokens.weight"), None)
-            out.g = None
-        self.tape.append(bwd)
+        def bwd(dy):
+            if self._tr("embed"):
+                T.embed_scatter_add(ids, dy.contiguous(), self._gm_scatter_target("model.embed_tokens.weight"), None)
+        self._backward(out, bwd)
         return out
 
     def splice(self, ids: torch.Tensor, vis: Optional[Var], n_vis: int) -> Var:
@@ -1064,16 +1052,13 @@ class TrainEngine:
         visv = vis.v.view(B, n_vis, E) if vis is not None else None
         out = Var(ops.embed_splice(ids, table, visv).view(B * Lx, E), self._tr("embed") or (vis is not None and vis.ng))
 
-        def bwd():
-            if out.g is None:
-                return
+        def bwd(dy):
             dvis = torch.empty(B * n_vis, E, device=self.dev, dtype=BF16) if (vis is not None and vis.ng) else None
-            T.embed_scatter_add(ids, out.g.contiguous(),
+            T.embed_scatter_add(ids, dy.contiguous(),
                                 self._gm_scatter_target("model.embed_tokens.weight") if self._tr("embed") else None, dvis, n_vis)
             if dvis is not None:
                 self._acc(vis, dvis, owned=True)
-            out.g = None
-        self.tape.append(bwd)
+        self._backward(out, bwd)
         return out
 
     def decoder(self, x: Var, B: int, Lx: int) -> Var:
@@ -1083,41 +1068,36 @@ class TrainEngine:
         g = self.g
         E, hq, hkv, dh, I = g.hidden_size, g.num_attention_heads, g.num_key_value_heads, g.head_dim, g.intermediate_size
         nh = hq + 2 * hkv
-        tr = self._tr("dec")
         eps = g.rms_norm_eps
 
         def layer(li, x):
             l = f"model.layers.{li}."
             self._mark([k for k in self.lay.mat_names if k.startswith(l)])
             y = self.rmsnorm(x, l + "input_layernorm.weight", "dec", eps)
-            qkv_raw = self._dec_linear(y, li, 0, tr)
-            qkv = self._rope_dec(qkv_raw, l, B, Lx)
+            qkv = self._rope_dec(self._dec_linear(y, li, 0), l, B, Lx)
             qv = lambda t: t.view(B, Lx, nh, dh)[:, :, :hq]
             kv_ = lambda t: t.view(B, Lx, nh, dh)[:, :, hq:hq + hkv]
             vv_ = lambda t: t.view(B, Lx, nh, dh)[:, :, hq + hkv:]
             ctx = self.attention(qkv, qv, qkv, kv_, qkv, vv_, (B, Lx, hq * dh), 1.0 / math.sqrt(dh), causal=True, group="dec",
                                  window=g.window)
-            c2 = Var(ctx.v.view(B * Lx, hq * dh), ctx.ng)
-            self._alias(c2, ctx)
-            x = self._dec_linear(c2, li, 1, tr, residual=x)
+            x = self._dec_linear(self._reshape(ctx, (B * Lx, hq * dh)), li, 1, residual=x)
             y = self.rmsnorm(x, l + "post_attention_layernorm.weight", "dec", eps)
-            gu = self._dec_linear(y, li, 2, tr)
-            act = self.silu_mul(gu)
-            return self._dec_linear(act, li, 3, tr, residual=x)
+            act = self.silu_mul(self._dec_linear(y, li, 2))
+            return self._dec_linear(act, li, 3, residual=x)
         for li in range(g.num_hidden_layers):
             x = self._segment(functools.partial(layer, li), x)
         return self.rmsnorm(x, "model.norm.weight", "dec", eps)
 
-    def _dec_linear(self, x: Var, li: int, gi: int, tr: bool, residual: Optional[Var] = None) -> Var:
+    def _dec_linear(self, x: Var, li: int, gi: int, residual: Optional[Var] = None) -> Var:
         """Fused group gi of lora_groups(g) of decoder layer li (q|k|v, o, gate|up, down). Without adapters: one linear
-        (wgrad when `tr`). With adapters on (some of) its members: the base output on the frozen weight, then for every
-        adapter j  U_j = s (D_j o x) A_j^T (lora_down) and y[:, rows_j] += U_j B_j^T on the GEMM (K = r)."""
+        (wgrad while the decoder trains). With adapters on (some of) its members: the base output on the frozen weight,
+        then for every adapter j  U_j = s (D_j o x) A_j^T (lora_down) and y[:, rows_j] += U_j B_j^T on the GEMM (K = r)."""
         pre, members = lora_groups(self.g)[gi]
         names = [f"model.layers.{li}.{pre}{t}.weight" for t in members]
         lo = self.lora
         tg = [t for t in members if lo is not None and t in lo.targets]
         if not tg:
-            return self.linear(x, self.wcat(names), self.gm(names) if tr else None, residual=residual)
+            return self._param_linear(x, names, None, "dec", residual=residual)
         if len(tg) != len(members):
             raise NotImplementedError(f"LoRA on part of a fused group ({tg} of {members}) is not supported on the training path")
         r, s = lo.r, lo.scaling
@@ -1142,10 +1122,7 @@ class TrainEngine:
             col += n
         out = Var(y, True)
 
-        def bwd():
-            dy = out.g
-            if dy is None:
-                return
+        def bwd(dy):
             dy2 = dy.view(-1, Ntot)
             dU = torch.empty_like(U)
             for j, (c0, n) in enumerate(cols):
@@ -1162,8 +1139,7 @@ class TrainEngine:
                 T.lora_dgrad(dU, A, x.g.view(-1, x2.shape[1]), r, s, p=p, seed=seed, streams=streams)
             if residual is not None:
                 self._acc(residual, dy, owned=True)
-            out.g = None
-        self.tape.append(bwd)
+        self._backward(out, bwd)
         return out
 
     def _rope_dec(self, qkv_raw: Var, l: str, B: int, Lx: int) -> Var:
@@ -1176,17 +1152,16 @@ class TrainEngine:
         ops.rope(y, rows=B * Lx, ld=nqkv, dh=dh, n_q=hq, n_k=hkv, n_v=0, inv_freq=self.inv_freq, q_norm_w=qn, k_norm_w=kn,
                  eps=g.rms_norm_eps, pos0=0, pos_div=1, pos_mod=Lx)
         out = Var(y, qkv_raw.ng)
-        tr = self._tr("dec")
+        dqn = dkn = None
+        if g.qk_norm and self._tr("dec"):
+            dqn, dkn = self.gv(l + "self_attn.q_norm.weight"), self.gv(l + "self_attn.k_norm.weight")
 
-        def bwd():
-            if out.g is not None and qkv_raw.ng:
-                T.rope_bwd(out.g, qkv_raw.v, rows=B * Lx, ld=nqkv, dh=dh, n_q=hq, n_k=hkv, inv_freq=self.inv_freq, q_norm_w=qn,
-                           k_norm_w=kn, eps=g.rms_norm_eps, pos0=0, pos_div=1, pos_mod=Lx,
-                           dq_norm_w=self.gv(l + "self_attn.q_norm.weight") if (qn is not None and tr) else None,
-                           dk_norm_w=self.gv(l + "self_attn.k_norm.weight") if (kn is not None and tr) else None)
-                self._acc(qkv_raw, out.g, owned=True)
-            out.g = None
-        self.tape.append(bwd)
+        def bwd(dy):
+            if qkv_raw.ng:
+                T.rope_bwd(dy, qkv_raw.v, rows=B * Lx, ld=nqkv, dh=dh, n_q=hq, n_k=hkv, inv_freq=self.inv_freq, q_norm_w=qn,
+                           k_norm_w=kn, eps=g.rms_norm_eps, pos0=0, pos_div=1, pos_mod=Lx, dq_norm_w=dqn, dk_norm_w=dkn)
+                self._acc(qkv_raw, dy, owned=True)
+        self._backward(out, bwd)
         return out
 
     def _head_w(self):
@@ -1217,7 +1192,7 @@ class TrainEngine:
                 self.wgrad(dl, h2, self.gm(hname))
             if hidden.ng:
                 self._acc(hidden, T.linear_dgrad(dl, Wh), owned=True)
-        self.tape.append(bwd)
+        self.tape.append((None, bwd))
         lin = "model.u2tokenizer.tta_module.layer_linagg.linear_aggregator."
         unused = [lin + "wv.weight", lin + "dense.weight"]   # never run by the reference either (tta.py:47-48,62-65)
         if not self.g.enable_diffts:
@@ -1257,26 +1232,26 @@ class TrainEngine:
             self._pending = [set(ns) for ns in self.lay.bucket_names]
         else:
             self._pending = None
-        for fn in reversed(self.tape):
-            fn()
+        self._run_tape(self.tape)
         self.tape = []
         self._pending = None
         self._gm_clear_stale(tuple(self._gm_dirty))   # whatever no marker covered
 
-    def _draw_lora_seed(self):
-        """LoRA dropout of a training forward: one nonzero 63-bit seed from torch's default generator (torch.manual_seed
-        makes the masks reproducible); the tape keeps it and the backward recomputes the masks from it."""
+    def _begin_pass(self, train: bool):
+        """Start a forward on an empty tape with fresh fp32 vector mirrors. A training pass draws the LoRA dropout seed (one
+        nonzero 63-bit seed from torch's default generator, so torch.manual_seed makes the masks reproducible; the backward
+        recomputes the masks from it) and checkpoints when `checkpoint` is set; a no-grad pass runs with neither."""
+        self.tape = []
+        self.refresh_vectors()
         self._lora_seed = 0
-        if self.lora is not None and self.lora.dropout > 0:
+        if train and self.lora is not None and self.lora.dropout > 0:
             self._lora_seed = int(torch.randint(1, 2 ** 63 - 1, (1,)).item())
+        self._ckpt = train and bool(self.checkpoint)
 
     def forward_loss(self, images, input_ids, question_ids, labels) -> torch.Tensor:
         """Forward half of the training step: HF ForCausalLMLoss of `model(images=, input_ids=, question_ids=, labels=)`
         (reference u2llama.py:76-87: shift by one, mean NLL over labels != -100). Keeps the tape for backward()."""
-        self.tape = []
-        self.refresh_vectors()
-        self._draw_lora_seed()
-        self._ckpt = bool(self.checkpoint)
+        self._begin_pass(train=True)
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         lab = labels.to(self.dev, torch.int64)
         shift = torch.full_like(lab, -100)
@@ -1303,10 +1278,7 @@ class TrainEngine:
         return loss
 
     def forward_loss_only(self, images, input_ids, question_ids, labels) -> torch.Tensor:
-        self.tape = []
-        self.refresh_vectors()
-        self._lora_seed = 0
-        self._ckpt = False
+        self._begin_pass(train=False)
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         lab = labels.to(self.dev, torch.int64)
         shift = torch.full_like(lab, -1)
@@ -1320,10 +1292,7 @@ class TrainEngine:
     def sequence_logps(self, images, input_ids, question_ids, loss_mask) -> torch.Tensor:
         """Summed log-probability of the masked tokens per sequence without gradients (the frozen reference model of the
         DPO step, trl DPOTrainer.compute_ref_log_probs / dpo_u2trainer.py:267-302)."""
-        self.tape = []
-        self.refresh_vectors()
-        self._lora_seed = 0
-        self._ckpt = False
+        self._begin_pass(train=False)
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         labels, mask = _dpo_labels(input_ids.to(self.dev), loss_mask.to(self.dev))
         hname, Wh = self._head_w()
@@ -1335,10 +1304,7 @@ class TrainEngine:
         """Policy side of the DPO step (reference dpo_u2trainer.py:185-359 + trl sigmoid loss, beta from
         train_stage2.py:83): rows [0, P) are the chosen, [P, 2P) the rejected sequences. ref_logps fp32 [2P] from the frozen
         reference model. Returns the fp32 [3] stats tensor (loss, reward accuracy, reward margin)."""
-        self.tape = []
-        self.refresh_vectors()
-        self._draw_lora_seed()
-        self._ckpt = bool(self.checkpoint)
+        self._begin_pass(train=True)
         hidden, B, Lx = self._forward_hidden(images, input_ids, question_ids)
         labels, mask = _dpo_labels(input_ids.to(self.dev), loss_mask.to(self.dev))
         stats = {}
@@ -1448,18 +1414,6 @@ class TrainEngine:
         T.adamw(o["v_master"], o["v_m"], o["v_v"], self.Gv, self.W[L.mat_total:L.mat_total + L.vec_total], param_out_f32=self.V32,
                 **kw)
         o["reduced"] = [False] * nb
-
-    def grads_for_module(self, model) -> None:
-        """p.grad views for the HF-style module (matrix grads alias Gm; vector grads are cast to bf16)."""
-        L = self.lay
-        self.sync_params()
-        gvb = torch.empty(L.vec_total, device=self.dev, dtype=BF16)
-        T.cast(self.Gv, gvb)
-        for n, p in model.named_parameters():
-            if n in L.mat_off:
-                p.grad = self.Gm[L.mat_off[n]:L.mat_off[n] + L._numel(n)].view(L.shapes[n])
-            elif n in L.vec_off:
-                p.grad = gvb[L.vec_off[n]:L.vec_off[n] + L._numel(n)].view(L.shapes[n])
 
 
 def _dpo_labels(input_ids: torch.Tensor, loss_mask: torch.Tensor):
