@@ -275,6 +275,8 @@ U2_API int u2_argmax_f32(const float* logits, int64_t* out, uint64_t* scratch, i
  * Replaces the HF decoder Linears at q_len == 1 (reference u2llama.py:123-126 -> GenerationMixin._sample). */
 #define U2_DLIN_STREAMK128 0
 #define U2_DLIN_TILES64 1
+#define U2_DLIN_W_BF16 0     /* w: bf16 [N, K], row stride ldw */
+#define U2_DLIN_W_PACKED13 1 /* w: the units u2_dlinear_pack_bf16 wrote (stream-K schedule only; ldw unused) */
 typedef struct u2_dlinear_desc {
   int32_t B, N, K;
   int64_t ldx, ldw, ldy, ldr, ldxg;
@@ -302,6 +304,7 @@ typedef struct u2_dlinear_desc {
   int32_t* out_flags;
   int32_t sched; /* U2_DLIN_STREAMK128 (128-row tiles, stream-K + workspace reduction) or
                     U2_DLIN_TILES64 (whole 64-row tiles per CTA, no inter-CTA reduction) */
+  int32_t w_format; /* U2_DLIN_W_BF16 or U2_DLIN_W_PACKED13; all ops of one multi-op launch share it */
 } u2_dlinear_desc;
 U2_API int u2_dlinear_bf16(const void* x, const void* w, void* y, const u2_dlinear_desc* desc, void* stream);
 U2_API int64_t u2_dlinear_ws_elems(int32_t N, int32_t K); /* fp32 elements of workspace for an N x K linear */
@@ -322,10 +325,18 @@ typedef struct u2_dlinear_next {
   int32_t N[2], K[2];
   int64_t ldw[2];
   int32_t units[2];
+  int32_t w_format[2];  /* U2_DLIN_W_BF16 or U2_DLIN_W_PACKED13 (w[j] then holds packed units; N, K as unpacked) */
 } u2_dlinear_next;
 U2_API int u2_dlinear_multi_bf16(const void* const* x, const void* const* w, void* const* y,
                                  const u2_dlinear_desc* descs, int32_t n_ops, uint32_t* gridbar,
                                  const int32_t* step_dev, int32_t pdl, const u2_dlinear_next* next, void* stream);
+/* Lossless 13-bit packing of a decode-linear weight w (bf16 [N, K], row stride ldw, K % 64 == 0) for the stream-K
+ * schedule: every 128 x 64 unit becomes 13 328 B (out: ceil(N / 128) * K / 64 units, 16-byte aligned). Per unit,
+ * base = max(emax - 31, 0) over the unit's exponent fields; an exponent e is stored as 0 when e == 0 and as e - base
+ * otherwise, sign and mantissa as they are, every plane in wgmma A-fragment order (layout: csrc/dlinear_wgmma.cu).
+ * Rows >= N are packed as +0. *bad (device int32) is incremented once per unit with a nonzero exponent <= base: a
+ * matrix with any such unit must stay in bf16. Unpacking reproduces every bf16 bit. */
+U2_API int u2_dlinear_pack_bf16(const void* w, int32_t N, int32_t K, int64_t ldw, void* out, int32_t* bad, void* stream);
 /* x[b] = table[ids[b]]; xg[b] = bf16(x * gamma); ssq[b] = sum x^2; ssq_zero[b] = 0; *step_counter += 1
  * (start of a decode step; step_counter may be NULL). Replaces `embed_tokens(input_ids)` of the cached decode step
  * (transformers models/qwen3/modeling_qwen3.py:392) + the first half of the first layer's input RMSNorm. */

@@ -100,6 +100,7 @@ class DlinearDesc(C.Structure):
         ("ws_elems", C.c_int64),
         ("dep_flags", C.c_void_p), ("dep_shift", C.c_int32), ("out_flags", C.c_void_p),
         ("sched", C.c_int32),
+        ("w_format", C.c_int32),
     ]
 
 
@@ -129,6 +130,7 @@ class DlinearNext(C.Structure):
         ("N", C.c_int32 * 2), ("K", C.c_int32 * 2),
         ("ldw", C.c_int64 * 2),
         ("units", C.c_int32 * 2),
+        ("w_format", C.c_int32 * 2),
     ]
 
 
@@ -290,6 +292,7 @@ SIGNATURES = {
     "u2_beam_step": (C.c_int, [C.POINTER(BeamStepDesc), _I, _P]),
     "u2_dlinear_ws_elems": (C.c_int64, [_I, _I]),
     "u2_dlinear_multi_bf16": (C.c_int, [_P, _P, _P, _P, _I, _P, _P, _I, _P, _P]),
+    "u2_dlinear_pack_bf16": (C.c_int, [_P, _I, _I, _L, _P, _P, _P]),
     "u2_preprocess_ws_bytes": (C.c_int64, [_I, _I, _I]),
     "u2_preprocess_volume_f32": (C.c_int, [_P, _P, _P, C.POINTER(PreprocessDesc), _P]),
     "u2_logprob_ws_bytes": (C.c_int64, [_I, _I]),

@@ -44,21 +44,64 @@ constexpr int kDlAccLd = 20;   // fp32 pitch of a handed-over accumulator row (1
 //                        inter-CTA reduction at all, so an op ends ~1 us after its last MMA. 64 rows x K is
 //                        still >= 0.5 MB per tile, and 64..96 active SMs already saturate HBM because one SM
 //                        can ingest far more than 1/132 of the HBM bandwidth through TMA.
-template <int kM>
+//
+// Packed weights (kPacked, kM = 128 only): one 128 x 64 unit is stored losslessly in 13 bits per weight, 13 328 B instead
+// of 16 KB, and streamed with one 1-D bulk copy. Per unit, base = max(emax - 31, 0) (emax: largest bf16 exponent field of
+// the unit); a weight's exponent e is coded as c = 0 when e = 0 (zeros, subnormals) and c = e - base (1..31) otherwise.
+// Layout (every plane in wgmma A-fragment order, interleaved [16-byte chunk][MMA thread] for conflict-free 16-byte loads;
+// thread t of the warpgroup owns 32 bf16x2 fragment words R = 16 mh + 4 ks + r, see unpack_word):
+//   [0, 16)          header: u32 base, 12 spare bytes
+//   [16, 8208)       s << 7 | m bytes: byte 2R + h of thread t at 16 + ((2R + h) / 16 * 128 + t) * 16 + (2R + h) % 16
+//   [8208, 12304)    low 4 code bits: word q = R / 4 of thread t holds word R's codes at bits 4 (R % 4) (column c) and
+//                    16 + 4 (R % 4) (column c + 1); word q at 8208 + (q / 4 * 128 + t) * 16 + 4 (q % 4)
+//   [12304, 13328)   high code bit: word u = R / 16 of thread t (at 12304 + 8 t + 4 u) holds bits R % 16 and 16 + R % 16
+// Units are stored tile-major ((tile * kblocks + kb) * 13 328 B), the order in which a CTA's stream-K range walks them.
+constexpr int kPkUnitBytes = 13328;
+constexpr int kPkSmOff = 16, kPkNibOff = 16 + 8192, kPkHiOff = 16 + 8192 + 4096;
+
+template <int kM, bool kPacked = false>
 struct DlCfg {
-  static constexpr int kABytes = kM * kDlK * 2;                 // 16 KB / 8 KB
+  static constexpr int kABytes = kPacked ? kPkUnitBytes : kM * kDlK * 2;  // 13 328 B / 16 KB / 8 KB
   static constexpr int kStageBytes = kABytes + kDlBBytes;
 #ifndef U2_DL_STAGES128
 #define U2_DL_STAGES128 10
 #endif
-  static constexpr int kStages = (kM == 128) ? U2_DL_STAGES128 : 18;  // <= ~180 KB of weight tiles in flight per SM
+  // <= ~180 KB of weight tiles in flight per SM (packed: 13 units of 13 328 B fill the same shared memory)
+  static constexpr int kStages = kPacked ? 13 : (kM == 128) ? U2_DL_STAGES128 : 18;
+  static constexpr int kBOff = (kStages * kABytes + 1023) & ~1023;  // B tiles 1024-byte aligned (128-byte swizzle)
+  static constexpr int kAccOff = kBOff + kStages * kDlBBytes;
   static constexpr int kAccBytes = 2 * kM * kDlAccLd * 4;      // double-buffered accumulator hand-over
-  static constexpr int kSmem = kStages * kStageBytes + kAccBytes + 1024 + 512;
+  static constexpr int kBarOff = kAccOff + kAccBytes;
+  static constexpr int kSmem = kBarOff + 512 + 1024;
+  static_assert(!kPacked || kM == 128, "packed weights use the 128-row stream-K schedule");
 };
+
+__device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t sel) {  // prmt.b32 (selector bit 3: replicate the sign)
+  uint32_t r;
+  asm("prmt.b32 %0, %1, 0, %2;" : "=r"(r) : "r"(a), "r"(sel));
+  return r;
+}
+
+// Fragment word R of a packed unit as the bf16x2 wgmma A operand. sm: the 32-bit word of s<<7|m bytes holding word R's
+// two bytes (bytes 0-1 for even R, 2-3 for odd R); nib / hi: this thread's code words covering R; b7 = (base << 7) in
+// both 16-bit halves. Every step works on both halves at once; no half carries into the other.
+template <int R>
+__device__ __forceinline__ uint32_t unpack_word(uint32_t sm, uint32_t nib, uint32_t hi, uint32_t b7) {
+  constexpr int i = R & 3, j = R & 15;
+  const uint32_t ns = (i < 2) ? (nib << (7 - 4 * i)) : (nib >> (4 * i - 7));
+  const uint32_t hs = (j <= 11) ? (hi << (11 - j)) : (hi >> (j - 11));
+  const uint32_t c7 = (ns & 0x07800780u) | (hs & 0x08000800u);  // code << 7 per half
+  // all-ones half where the code is not 0: bit 15 of (c7 + 0x7f80) is set iff c7 >= 0x80, replicated by byte permute
+  const uint32_t nz = prmt(c7 + 0x7f807f80u, 0xBB99u);
+  const uint32_t e7 = c7 + (nz & b7);                           // exponent field << 7
+  const uint32_t z = prmt(sm, (R & 1) ? 0x3322u : 0x1100u);  // byte b in both bytes of its half
+  return (z & 0x807f807fu) | e7;                                // sign (bit 7 of the high copy) | mantissa | exponent
+}
 
 struct DlinArgs {
   int B, N, K;                 // sequences, output rows of W, reduction length
   int num_tiles, kblocks;      // ceil(N/kM), K/64
+  const uint8_t* wpk;          // packed weight units (kPacked launches; the tensor map is unused then)
   float* ws;                   // [num_tiles][max_slots][kM][16] fp32 partial-sum slots (stream-K schedule only);
                                // every word holds the sentinel 0xffffffff between uses
   int max_slots;
@@ -100,6 +143,7 @@ struct DlinMulti {
   // issued when this launch has nothing left to load, so HBM keeps working through our tail, the launch gap
   // and the attention kernel in between.
   CUtensorMap tnext[2];
+  const uint8_t* next_pk[2];  // packed next weights (else null: tnext)
   int next_tiles[2], next_kblocks[2], next_units[2];  // next_units: how many leading units per CTA to prefetch
   int n_next;
   int pre_stages;             // ring stages filled with the next op's weights before its dependency resolves
@@ -136,15 +180,13 @@ __device__ __forceinline__ float4 ld_relaxed_f4(const float4* p) {
 // the occupancy calculator). If something outside this library takes SMs away for good (an MPS active-thread limit,
 // a kernel of another context that never ends), the missing CTAs never arrive: after ~2^24 L2 round trips (seconds;
 // a healthy wait is tens of microseconds) the poller traps, so the step fails loudly instead of hanging the GPU.
+// No printf here: any function call in the kernel makes ptxas serialize every wgmma (C7510: a wait after each one),
+// which made the MMA warpgroup, not HBM, set the pace of the weight stream.
 __device__ __forceinline__ void grid_barrier_wait(const unsigned int* bar, unsigned int target) {
   unsigned int v, spins = 0;
   do {
     asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory");
-    if (++spins == (1u << 24)) {
-      printf("u2 dlinear: grid barrier timed out (CTA %d sees %u of %u arrivals): CTAs of the launch are not co-resident\n",
-             (int)blockIdx.x, v, target);
-      __trap();
-    }
+    if (++spins == (1u << 24)) __trap();  // CTAs of the launch are not co-resident
   } while (v < target);
   asm volatile("fence.acq_rel.gpu;" ::: "memory");
 }
@@ -222,10 +264,10 @@ __device__ __forceinline__ void wait_tile_flag(const int* flags, int t, int step
 // layer's qkv): between two linears all CTAs meet at a software grid barrier, but the TMA producer keeps
 // the smem ring full with the NEXT linear's weight tiles while the current one drains and finalises, so the
 // HBM stream barely pauses at the dependency.
-template <int kM>
+template <int kM, bool kPacked>
 __global__ void __launch_bounds__(kDlThreads, 1)
 dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
-  using Cfg = DlCfg<kM>;
+  using Cfg = DlCfg<kM, kPacked>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kABytes = Cfg::kABytes;
   constexpr int kStageBytes = Cfg::kStageBytes;
@@ -233,9 +275,9 @@ dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kStages * kABytes;
-  float* smem_acc = reinterpret_cast<float*>(smem + kStages * kStageBytes);  // [2][kM][kDlAccLd]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes + Cfg::kAccBytes);
+  uint8_t* smem_b = smem + Cfg::kBOff;
+  float* smem_acc = reinterpret_cast<float*>(smem + Cfg::kAccOff);  // [2][kM][kDlAccLd]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kBarOff);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
   uint64_t* acc_full_bar = bars + 2 * kStages;
@@ -249,7 +291,7 @@ dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
 
   if (warp_idx == 0 && lane == 0) {
     for (int i = 0; i < n_ops; ++i) {
-      tma_prefetch_desc(&mp.tw[i]);
+      if (!kPacked) tma_prefetch_desc(&mp.tw[i]);
       tma_prefetch_desc(&mp.tx[i]);
     }
   }
@@ -276,6 +318,14 @@ dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
       // every weight byte is read once per token: weight tiles are the first lines L2 gives up, so the streamed weights
       // do not push out what is read again (activations, split-tile slots, counters, the attention's KV cache)
       const uint64_t pol_w = l2_policy_evict_first();
+      // weight half of a stage: one packed unit (1-D bulk copy) or one 128B-swizzled bf16 tile (tensor map)
+      auto load_w = [&](int st, const DlinArgs& p, int oi, const UnitIter& u) {
+        if constexpr (kPacked)
+          bulk_load_hint(smem_a + st * kABytes, p.wpk + ((long long)u.tile * u.kblocks + u.kb) * kPkUnitBytes,
+                         kPkUnitBytes, &full_bar[st], pol_w);
+        else
+          tma_load_4d_hint(smem_a + st * kABytes, &mp.tw[oi], &full_bar[st], u.kb * kDlK, u.tile * kM, 0, 0, pol_w);
+      };
       int stage = 0;
       uint32_t phase = 0;
       unsigned int target = 0;
@@ -295,7 +345,7 @@ dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
         for (int j = 0; j < npre; ++j) {
           mbar_wait(&empty_bar[st], ph ^ 1);
           mbar_arrive_expect_tx(&full_bar[st], kStageBytes);
-          tma_load_4d_hint(smem_a + st * kABytes, &mp.tw[oi], &full_bar[st], pre.kb * kDlK, pre.tile * kM, 0, 0, pol_w);
+          load_w(st, p, oi, pre);
           pre.next();
           if (++st == kStages) {
             st = 0;
@@ -306,7 +356,10 @@ dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
         {
           UnitIter la = pre;
           for (int j = 0; j < mp.lookahead_units && la.left > 0; ++j) {
-            tma_prefetch_l2_4d(&mp.tw[oi], la.kb * kDlK, la.tile * kM, 0, 0);
+            if constexpr (kPacked)
+              bulk_prefetch_l2(p.wpk + ((long long)la.tile * la.kblocks + la.kb) * kPkUnitBytes, kPkUnitBytes);
+            else
+              tma_prefetch_l2_4d(&mp.tw[oi], la.kb * kDlK, la.tile * kM, 0, 0);
             la.next();
           }
         }
@@ -336,7 +389,7 @@ dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
         while (it.left > 0) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
-          tma_load_4d_hint(smem_a + stage * kABytes, &mp.tw[oi], &full_bar[stage], it.kb * kDlK, it.tile * kM, 0, 0, pol_w);
+          load_w(stage, p, oi, it);
           if (oi > 0 && p.dep_flags) wait_tile_flag(p.dep_flags, it.kb >> p.dep_shift, step, s_ready, oi);
           tma_load_4d(smem_b + stage * kDlBBytes, &mp.tx[oi], &full_bar[stage], it.kb * kDlK, 0, 0, 0);
           it.next();
@@ -350,7 +403,10 @@ dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
       for (int jn = 0; jn < mp.n_next; ++jn) {
         UnitIter la = make_iter(mp.next_tiles[jn], mp.next_kblocks[jn], kTiles);
         for (int j = 0; j < mp.next_units[jn] && la.left > 0; ++j) {
-          tma_prefetch_l2_4d(&mp.tnext[jn], la.kb * kDlK, la.tile * kM, 0, 0);
+          if (mp.next_pk[jn])
+            bulk_prefetch_l2(mp.next_pk[jn] + ((long long)la.tile * la.kblocks + la.kb) * kPkUnitBytes, kPkUnitBytes);
+          else
+            tma_prefetch_l2_4d(&mp.tnext[jn], la.kb * kDlK, la.tile * kM, 0, 0);
           la.next();
         }
       }
@@ -374,14 +430,52 @@ dlinear_wgmma_kernel(const __grid_constant__ DlinMulti mp) {
             if (threadIdx.x == kDlMmaWarp0 * 32) U2_STAMP(oi, 2);  // first stage of the op landed
             first_unit = false;
           }
-          const uint64_t a_desc = gmma_desc_sw128(smem_u32(smem_a + stage * kABytes));
           const uint64_t b_desc = gmma_desc_sw128(smem_u32(smem_b + stage * kDlBBytes));
-          wgmma_fence();
+          if constexpr (kPacked) {
+            // this thread's 104 bytes of the unit -> its 32 bf16x2 A-fragment words (bit-identical to the bf16 weights)
+            const uint32_t ua = smem_u32(smem_a + stage * kABytes);
+            const uint32_t t16 = (threadIdx.x - kDlMmaWarp0 * 32) * 16;
+            uint32_t smw[16], nib[8], hi[2];
+            const uint32_t base = lds128(ua).x;
 #pragma unroll
-          for (int k = 0; k < kDlK / 16; ++k) {
+            for (int c = 0; c < 4; ++c) {
+              const uint4 v = lds128(ua + kPkSmOff + c * 2048 + t16);
+              smw[4 * c] = v.x; smw[4 * c + 1] = v.y; smw[4 * c + 2] = v.z; smw[4 * c + 3] = v.w;
+            }
 #pragma unroll
-            for (int mh = 0; mh < kM / 64; ++mh)  // weight rows 64..127 start 8 KB further
-              wgmma_m64n16k16_ss(d[mh], a_desc + 512 * mh + 2 * k, b_desc + 2 * k, (j == 0 && k == 0) ? 0u : 1u);
+            for (int c = 0; c < 2; ++c) {
+              const uint4 v = lds128(ua + kPkNibOff + c * 2048 + t16);
+              nib[4 * c] = v.x; nib[4 * c + 1] = v.y; nib[4 * c + 2] = v.z; nib[4 * c + 3] = v.w;
+            }
+            {
+              uint2 v;
+              asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(ua + kPkHiOff + t16 / 2));
+              hi[0] = v.x; hi[1] = v.y;
+            }
+            const uint32_t b7 = (base << 7) * 0x10001u;
+            uint32_t a[8][4];  // [mh * 4 + ks][r]
+#define U2_PK_W(R) a[(R) >> 2][(R) & 3] = unpack_word<R>(smw[(R) >> 1], nib[(R) >> 2], hi[(R) >> 4], b7)
+            U2_PK_W(0); U2_PK_W(1); U2_PK_W(2); U2_PK_W(3); U2_PK_W(4); U2_PK_W(5); U2_PK_W(6); U2_PK_W(7);
+            U2_PK_W(8); U2_PK_W(9); U2_PK_W(10); U2_PK_W(11); U2_PK_W(12); U2_PK_W(13); U2_PK_W(14); U2_PK_W(15);
+            U2_PK_W(16); U2_PK_W(17); U2_PK_W(18); U2_PK_W(19); U2_PK_W(20); U2_PK_W(21); U2_PK_W(22); U2_PK_W(23);
+            U2_PK_W(24); U2_PK_W(25); U2_PK_W(26); U2_PK_W(27); U2_PK_W(28); U2_PK_W(29); U2_PK_W(30); U2_PK_W(31);
+#undef U2_PK_W
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kDlK / 16; ++k) {
+#pragma unroll
+              for (int mh = 0; mh < kM / 64; ++mh)
+                wgmma_m64n16k16_rs(d[mh], a[mh * 4 + k], b_desc + 2 * k, (j == 0 && k == 0) ? 0u : 1u);
+            }
+          } else {
+            const uint64_t a_desc = gmma_desc_sw128(smem_u32(smem_a + stage * kABytes));
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kDlK / 16; ++k) {
+#pragma unroll
+              for (int mh = 0; mh < kM / 64; ++mh)  // weight rows 64..127 start 8 KB further
+                wgmma_m64n16k16_ss(d[mh], a_desc + 512 * mh + 2 * k, b_desc + 2 * k, (j == 0 && k == 0) ? 0u : 1u);
+            }
           }
           wgmma_commit();
           wgmma_wait<0>();
@@ -701,6 +795,63 @@ decode_embed_kernel(const long long* __restrict__ ids, const __nv_bfloat16* __re
   }
 }
 
+// Packs one 128 x 64 unit per CTA (128 threads, thread t = the MMA thread that will unpack its 64 weights) into the
+// layout described at kPkUnitBytes. A unit whose exponents do not fit the code (a nonzero exponent at or below base)
+// is counted in *bad; its bytes are then meaningless and the caller keeps the bf16 weights.
+__global__ void __launch_bounds__(128)
+dlinear_pack_kernel(const uint16_t* __restrict__ w, long long ldw, int N, int kblocks, uint8_t* __restrict__ out,
+                    int* __restrict__ bad) {
+  const int unit = blockIdx.x, tile = unit / kblocks, kb = unit - tile * kblocks;
+  const int t = threadIdx.x, wq = t >> 5, l = t & 31;
+  uint32_t v[32];  // fragment word R: (column c, column c + 1) bf16 pair
+  int emax = 0;
+#pragma unroll
+  for (int R = 0; R < 32; ++R) {
+    const int mh = R >> 4, ks = (R >> 2) & 3, r = R & 3;
+    const int row = tile * 128 + mh * 64 + wq * 16 + (l >> 2) + 8 * (r & 1);
+    const int col = kb * kDlK + ks * 16 + 2 * (l & 3) + 8 * (r >> 1);
+    v[R] = row < N ? *reinterpret_cast<const uint32_t*>(w + (long long)row * ldw + col) : 0u;
+    emax = max(emax, (int)max((v[R] >> 7) & 0xff, (v[R] >> 23) & 0xff));
+  }
+  __shared__ int s_max[4];
+  __shared__ int s_bad;
+  emax = __reduce_max_sync(0xffffffffu, emax);
+  if (l == 0) s_max[wq] = emax;
+  if (t == 0) s_bad = 0;
+  __syncthreads();
+  emax = max(max(s_max[0], s_max[1]), max(s_max[2], s_max[3]));
+  const int base = emax > 31 ? emax - 31 : 0;
+  uint32_t smw[16] = {}, nib[8] = {}, hi[2] = {};
+  bool fits = true;
+#pragma unroll
+  for (int R = 0; R < 32; ++R) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t x = (v[R] >> (16 * h)) & 0xffffu;
+      const int e = (x >> 7) & 0xff;
+      fits = fits && (e == 0 || e > base);
+      const uint32_t c = e == 0 ? 0u : (uint32_t)(e - base) & 31u;
+      smw[R >> 1] |= (((x >> 8) & 0x80u) | (x & 0x7fu)) << (8 * (2 * (R & 1) + h));
+      nib[R >> 2] |= (c & 15u) << (4 * (R & 3) + 16 * h);
+      hi[R >> 4] |= (c >> 4) << ((R & 15) + 16 * h);
+    }
+  }
+  if (!fits) s_bad = 1;
+  uint8_t* u = out + (long long)unit * kPkUnitBytes;
+  if (t == 0) *reinterpret_cast<uint4*>(u) = make_uint4((uint32_t)base, 0u, 0u, 0u);
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+    *reinterpret_cast<uint4*>(u + kPkSmOff + (c * 128 + t) * 16) =
+        make_uint4(smw[4 * c], smw[4 * c + 1], smw[4 * c + 2], smw[4 * c + 3]);
+#pragma unroll
+  for (int c = 0; c < 2; ++c)
+    *reinterpret_cast<uint4*>(u + kPkNibOff + (c * 128 + t) * 16) =
+        make_uint4(nib[4 * c], nib[4 * c + 1], nib[4 * c + 2], nib[4 * c + 3]);
+  *reinterpret_cast<uint2*>(u + kPkHiOff + t * 8) = make_uint2(hi[0], hi[1]);
+  __syncthreads();
+  if (t == 0 && s_bad) atomicAdd(bad, 1);
+}
+
 }  // namespace u2
 
 using namespace u2;
@@ -710,12 +861,17 @@ static int fill_op(const void* x, const void* w, void* y, const u2_dlinear_desc*
   if (!x || !w || !y || !d || !d->ws || !d->counters) return set_error(U2_ERR_ARG, "dlinear: null pointer");
   if (d->B < 1 || d->B > kDlN) return set_error(U2_ERR_UNSUPPORTED, "dlinear: 1 <= B <= 16 (got %d)", d->B);
   if (d->N <= 0 || d->K <= 0 || (d->K % kDlK)) return set_error(U2_ERR_ARG, "dlinear: K must be a positive multiple of 64");
-  if ((d->ldx & 7) || (d->ldw & 7)) return set_error(U2_ERR_ARG, "dlinear: ldx/ldw must be multiples of 8");
+  const bool packed = d->w_format == U2_DLIN_W_PACKED13;
+  if (!packed && d->w_format != U2_DLIN_W_BF16) return set_error(U2_ERR_ARG, "dlinear: unknown w_format %d", d->w_format);
+  if (packed && kM != 128) return set_error(U2_ERR_UNSUPPORTED, "dlinear: packed weights need the stream-K schedule");
+  if (packed && (reinterpret_cast<uintptr_t>(w) & 15)) return set_error(U2_ERR_ARG, "dlinear: packed weights must be 16-byte aligned");
+  if ((d->ldx & 7) || (!packed && (d->ldw & 7))) return set_error(U2_ERR_ARG, "dlinear: ldx/ldw must be multiples of 8");
   if (d->silu_pair && (d->N & 1)) return set_error(U2_ERR_ARG, "dlinear: silu_pair needs an even N");
   if (d->gamma_next && !d->xg) return set_error(U2_ERR_ARG, "dlinear: gamma_next needs xg");
   p->B = d->B; p->N = d->N; p->K = d->K;
   p->num_tiles = (d->N + kM - 1) / kM;
   p->kblocks = d->K / kDlK;
+  p->wpk = packed ? reinterpret_cast<const uint8_t*>(w) : nullptr;
   p->ws = d->ws; p->counters = d->counters;
   p->max_slots = 1;
   if (kM == 128) {
@@ -758,20 +914,24 @@ static int fill_op(const void* x, const void* w, void* y, const u2_dlinear_desc*
   p->dep_shift = d->dep_shift;
   p->out_flags = d->out_flags;
   p->dbg = nullptr;
-  int rc = make_tmap_bf16_4d(tw, w, d->K, d->N, 1, 1, d->ldw, 0, 0, kDlK, kM);
-  if (rc) return rc;
+  if (!packed) {
+    int rc = make_tmap_bf16_4d(tw, w, d->K, d->N, 1, 1, d->ldw, 0, 0, kDlK, kM);
+    if (rc) return rc;
+  }
   return make_tmap_bf16_4d(tx, x, d->K, d->B, 1, 1, d->ldx, 0, 0, kDlK, kDlN);
 }
 
-template <int kM>
+template <int kM, bool kPacked>
 static int launch_multi_t(DlinMulti& mp, int pdl, cudaStream_t stream) {
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(dlinear_wgmma_kernel<kM>, cudaFuncAttributeMaxDynamicSharedMemorySize, DlCfg<kM>::kSmem);
+    cudaError_t e = cudaFuncSetAttribute(dlinear_wgmma_kernel<kM, kPacked>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         DlCfg<kM, kPacked>::kSmem);
     if (e != cudaSuccess) return set_error(U2_ERR_CUDA, "dlinear: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     // the software grid barrier between the chained linears needs grid <= resident CTA capacity
     int per_sm = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dlinear_wgmma_kernel<kM>, kDlThreads, DlCfg<kM>::kSmem);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dlinear_wgmma_kernel<kM, kPacked>, kDlThreads,
+                                                      DlCfg<kM, kPacked>::kSmem);
     if (e != cudaSuccess || per_sm < 1)
       return set_error(U2_ERR_CUDA, "dlinear: kernel cannot be resident on an SM (%s, %d CTA/SM): set U2_MULTI_OP=0",
                        cudaGetErrorString(e), per_sm);
@@ -786,20 +946,21 @@ static int launch_multi_t(DlinMulti& mp, int pdl, cudaStream_t stream) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)grid);
   cfg.blockDim = dim3(kDlThreads);
-  cfg.dynamicSmemBytes = DlCfg<kM>::kSmem;
+  cfg.dynamicSmemBytes = DlCfg<kM, kPacked>::kSmem;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, dlinear_wgmma_kernel<kM>, mp);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, dlinear_wgmma_kernel<kM, kPacked>, mp);
   if (e != cudaSuccess) return set_error(U2_ERR_CUDA, "dlinear launch: %s", cudaGetErrorString(e));
   return U2_OK;
 }
 
-static int launch_multi(DlinMulti& mp, int kM, int pdl, cudaStream_t stream) {
-  return kM == 64 ? launch_multi_t<64>(mp, pdl, stream) : launch_multi_t<128>(mp, pdl, stream);
+static int launch_multi(DlinMulti& mp, int kM, bool packed, int pdl, cudaStream_t stream) {
+  if (packed) return launch_multi_t<128, true>(mp, pdl, stream);
+  return kM == 64 ? launch_multi_t<64, false>(mp, pdl, stream) : launch_multi_t<128, false>(mp, pdl, stream);
 }
 
 static inline int tile_m_of(const u2_dlinear_desc* d) { return d->sched == U2_DLIN_TILES64 ? 64 : 128; }
@@ -831,7 +992,7 @@ extern "C" U2_API int u2_dlinear_bf16(const void* x, const void* w, void* y, con
   // single op: the step counter is only read to form a barrier target that is never used; point it at any
   // valid device int (the tile counters are zero between launches)
   mp.step_dev = d->counters;
-  return launch_multi(mp, kM, d->pdl, reinterpret_cast<cudaStream_t>(stream));
+  return launch_multi(mp, kM, d->w_format == U2_DLIN_W_PACKED13, d->pdl, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" U2_API int u2_dlinear_multi_bf16(const void* const* x, const void* const* w, void* const* y,
@@ -844,8 +1005,10 @@ extern "C" U2_API int u2_dlinear_multi_bf16(const void* const* x, const void* co
   static DlinMulti mp;
   mp.n_ops = n_ops;
   const int kM = tile_m_of(&descs[0]);
+  const int32_t fmt = descs[0].w_format;
   for (int i = 0; i < n_ops; ++i) {
     if (tile_m_of(&descs[i]) != kM) return set_error(U2_ERR_ARG, "dlinear_multi: all ops of a launch must share one schedule");
+    if (descs[i].w_format != fmt) return set_error(U2_ERR_ARG, "dlinear_multi: all ops of a launch must share one weight format");
     int rc = fill_op(x[i], w[i], y[i], &descs[i], &mp.op[i], &mp.tw[i], &mp.tx[i], kM);
     if (rc) return rc;
   }
@@ -856,8 +1019,14 @@ extern "C" U2_API int u2_dlinear_multi_bf16(const void* const* x, const void* co
   if (next) {
     for (int j = 0; j < 2 && j < next->n; ++j) {
       if (!next->w[j] || next->K[j] % kDlK || next->N[j] <= 0) return set_error(U2_ERR_ARG, "dlinear_multi: bad look-ahead weight");
-      int rc = make_tmap_bf16_4d(&mp.tnext[j], next->w[j], next->K[j], next->N[j], 1, 1, next->ldw[j], 0, 0, kDlK, kM);
-      if (rc) return rc;
+      mp.next_pk[j] = nullptr;
+      if (next->w_format[j] == U2_DLIN_W_PACKED13) {
+        if (kM != 128) return set_error(U2_ERR_UNSUPPORTED, "dlinear_multi: packed look-ahead needs the stream-K schedule");
+        mp.next_pk[j] = reinterpret_cast<const uint8_t*>(next->w[j]);
+      } else {
+        int rc = make_tmap_bf16_4d(&mp.tnext[j], next->w[j], next->K[j], next->N[j], 1, 1, next->ldw[j], 0, 0, kDlK, kM);
+        if (rc) return rc;
+      }
       mp.next_tiles[j] = (next->N[j] + kM - 1) / kM;
       mp.next_kblocks[j] = next->K[j] / kDlK;
       mp.next_units[j] = next->units[j];
@@ -866,7 +1035,20 @@ extern "C" U2_API int u2_dlinear_multi_bf16(const void* const* x, const void* co
   }
   mp.dbg = reinterpret_cast<unsigned long long*>(descs[0].dbg);
   mp.step_dev = step_dev ? step_dev : descs[0].counters;
-  return launch_multi(mp, kM, pdl, reinterpret_cast<cudaStream_t>(stream));
+  return launch_multi(mp, kM, fmt == U2_DLIN_W_PACKED13, pdl, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" U2_API int u2_dlinear_pack_bf16(const void* w, int32_t N, int32_t K, int64_t ldw, void* out, int32_t* bad,
+                                           void* stream) {
+  if (!w || !out || !bad) return set_error(U2_ERR_ARG, "dlinear_pack: null pointer");
+  if (N <= 0 || K <= 0 || K % kDlK) return set_error(U2_ERR_ARG, "dlinear_pack: K must be a positive multiple of 64");
+  if (ldw < K || (ldw & 1) || (reinterpret_cast<uintptr_t>(w) & 3) || (reinterpret_cast<uintptr_t>(out) & 15))
+    return set_error(U2_ERR_ARG, "dlinear_pack: ldw >= K and even, w 4-byte and out 16-byte aligned");
+  const long long units = (long long)((N + 127) / 128) * (K / kDlK);
+  dlinear_pack_kernel<<<(unsigned)units, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const uint16_t*>(w), ldw, N, K / kDlK, reinterpret_cast<uint8_t*>(out), bad);
+  U2_CHECK_LAUNCH("dlinear_pack");
+  return U2_OK;
 }
 
 extern "C" U2_API int u2_decode_embed_bf16(const int64_t* ids, const void* table, const float* gamma, void* x,

@@ -127,6 +127,22 @@ __device__ __forceinline__ void tma_load_4d_hint(void* smem_dst, const CUtensorM
       : "memory");
 }
 
+// 1-D bulk copy global -> shared of `bytes` (multiple of 16, both addresses 16-byte aligned) with an L2 cache policy,
+// completing on mbar.
+__device__ __forceinline__ void bulk_load_hint(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar,
+                                               uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+      :
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+      : "memory");
+}
+
+// L2 prefetch of a contiguous global range (multiple of 16 bytes, 16-byte aligned).
+__device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(src)), "r"(bytes) : "memory");
+}
+
 // 3-D tiled load (used by the patch-embed brick gather).
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
                                             int c0, int c1, int c2) {
@@ -224,6 +240,21 @@ __device__ __forceinline__ void wgmma_m64n16k16_ss(float (&d)[8], uint64_t a_des
       "}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
       : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
+// Same with A taken from registers: a[0..3] is this thread's m64k16 A fragment (bf16x2 words: rows r, r + 8 at columns
+// c, c + 1, then rows r, r + 8 at columns c + 8, c + 9; r = 16 w + l / 4, c = 2 (l % 4)).
+__device__ __forceinline__ void wgmma_m64n16k16_rs(float (&d)[8], const uint32_t (&a)[4], uint64_t b_desc,
+                                                   uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
 }
 
 // Accumulator fragment of an m64nN wgmma: element j of this thread (warp w of the warpgroup, lane l) holds

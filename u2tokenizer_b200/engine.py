@@ -307,6 +307,18 @@ class U2Engine:
         self.final_norm = t.f32("model.norm.weight")
         self.lm_head = self.embed if (g.tie_word_embeddings or not t.has("lm_head.weight")) else t.bf("lm_head.weight")
         self.inv_freq = self._decoder_inv_freq().to(self.dev)
+        # The decode step streams every weight once per token, so it reads the lossless 13-bit packing of each matrix
+        # that fits it (ops.dlinear_pack: 0.81 of the bf16 bytes); prefill and training keep the bf16 copies. A tied
+        # head's packed copy serves the decode head only. Keys: (layer, name) and ("head",).
+        self._packed = {}
+        if self.decode_impl == "tcgen05" and all(
+                k % 64 == 0 for k in (g.hidden_size, g.intermediate_size, g.num_attention_heads * g.head_dim)):
+            mats = [((i, k), l[k]) for i, l in enumerate(self.layers) for k in ("wqkv", "wo", "wgu", "wdown")]
+            for key, w in mats + [(("head",), self.lm_head)]:
+                pk = ops.dlinear_pack(w)
+                if pk is not None:
+                    self._packed[key] = pk
+        self._decode_bf16 = False  # True: the decode step streams the bf16 weights (reference runs and A/B measurements)
 
     def _decoder_inv_freq(self) -> torch.Tensor:
         """Default RoPE or the llama3 rescaling (HF modeling_rope_utils; reference config.json:49-56)."""
@@ -758,8 +770,17 @@ class U2Engine:
         nl = len(self.layers)
         c0 = dict(ws=ws[0], counters=cnt[0], sched=self.dl_sched)
         c1 = dict(ws=ws[1], counters=cnt[1], sched=self.dl_sched)
+        packed = {} if (self._decode_bf16 or self.dl_sched != 0) else self._packed  # the kM = 64 schedule reads bf16
+
+        def launch_w(keys):
+            """One launch's weights: all packed when every one of them is, else all bf16 (a launch has one format)."""
+            pk = [packed.get(k) for k in keys]
+            if all(p is not None for p in pk):
+                return pk
+            return [self.lm_head if k == ("head",) else self.layers[k[0]][k[1]] for k in keys]
+
         ops.decode_embed(ids, self.embed, self.layers[0]["ln1"], x, xg_b, ssq_b, ssq_a, step)
-        ops.dlinear(xg_b, self.layers[0]["wqkv"], qkv, ssq_in=ssq_b, eps=eps, pdl=self.pdl, **c1)
+        ops.dlinear(xg_b, launch_w([(0, "wqkv")])[0], qkv, ssq_in=ssq_b, eps=eps, pdl=self.pdl, **c1)
         for li, w in enumerate(self.layers):
             ops.decode_attention_fused(qkv, cache.k[li], cache.v[li], ctx, B=B, Hq=hq, Hkv=hkv, dh=dh, Tmax=cache.max_len,
                                        inv_freq=self.inv_freq, scale=1.0 / math.sqrt(dh), pos_dev=cache.length_dev,
@@ -770,19 +791,19 @@ class U2Engine:
             g_next = self.final_norm if last else self.layers[li + 1]["ln1"]
             fl = flags[li] if (self.multi_op and self.fine_deps) else [None] * 4
             dep = lambda i, shift: dict(dep_flags=fl[i], dep_shift=shift) if fl[i] is not None else {}
+            wo, wgu, wdown, wnext = launch_w([(li, "wo"), (li, "wgu"), (li, "wdown"), ("head",) if last else (li + 1, "wqkv")])
             chain = [
-                (ctx, w["wo"], x, dict(residual=x, gamma_next=w["ln2"], xg=xg_a, ssq_out=ssq_a, ssq_zero=ssq_b,
-                                       out_flags=fl[0], **c0)),
-                (xg_a, w["wgu"], act, dict(ssq_in=ssq_a, eps=eps, silu_pair=True, out_flags=fl[1], **dep(0, 1), **c1)),
-                (act, w["wdown"], x, dict(residual=x, gamma_next=g_next, xg=xg_b, ssq_out=ssq_b, ssq_zero=ssq_a,
-                                          out_flags=fl[2], **dep(1, 0), **c0)),
-                (xg_b, self.lm_head, logits, dict(ssq_in=ssq_b, eps=eps, **dep(2, 1), **c1)) if last else
-                (xg_b, self.layers[li + 1]["wqkv"], qkv, dict(ssq_in=ssq_b, eps=eps, **dep(2, 1), **c1)),
+                (ctx, wo, x, dict(residual=x, gamma_next=w["ln2"], xg=xg_a, ssq_out=ssq_a, ssq_zero=ssq_b,
+                                  out_flags=fl[0], **c0)),
+                (xg_a, wgu, act, dict(ssq_in=ssq_a, eps=eps, silu_pair=True, out_flags=fl[1], **dep(0, 1), **c1)),
+                (act, wdown, x, dict(residual=x, gamma_next=g_next, xg=xg_b, ssq_out=ssq_b, ssq_zero=ssq_a,
+                                     out_flags=fl[2], **dep(1, 0), **c0)),
+                (xg_b, wnext, logits if last else qkv, dict(ssq_in=ssq_b, eps=eps, **dep(2, 1), **c1)),
             ]
             if self.multi_op:
                 # L2 look-ahead: next layer's o_proj (all of it) and the head of its gate|up stream
-                nxt = () if (last or self.l2_next_units < 0) else (
-                    (self.layers[li + 1]["wo"], 1 << 20), (self.layers[li + 1]["wgu"], self.l2_next_units))
+                nxt = () if (last or self.l2_next_units < 0) else tuple(
+                    zip(launch_w([(li + 1, "wo"), (li + 1, "wgu")]), (1 << 20, self.l2_next_units)))
                 ops.dlinear_multi(chain, gridbar=gridbar[li * 4:(li + 1) * 4], step_dev=step, pdl=self.pdl,
                                   lookahead_units=self.l2_lookahead_units, next_weights=nxt,
                                   pre_stages=self.pre_stages)

@@ -404,16 +404,56 @@ def argmax(logits: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Te
     return out
 
 
+DLIN_W_BF16, DLIN_W_PACKED13 = 0, 1  # U2_DLIN_W_* of include/u2b200.h
+DLIN_PACKED_UNIT_BYTES = 13328       # one packed 128 x 64 unit
+
+
+class PackedWeight:
+    """A decode-linear weight in the lossless 13-bit packing of u2_dlinear_pack_bf16: ``buf`` holds the units of the
+    [N, K] bf16 matrix it was made from (uint8, ceil(N / 128) * K / 64 * 13 328 bytes)."""
+
+    def __init__(self, buf: torch.Tensor, N: int, K: int):
+        self.buf, self.N, self.K = buf, N, K
+
+    @property
+    def shape(self):
+        return (self.N, self.K)
+
+
+def dlinear_pack(w: torch.Tensor) -> Optional[PackedWeight]:
+    """Pack a bf16 [N, K] weight (K % 64 == 0) for ops.dlinear / ops.dlinear_multi. Returns None when a 128 x 64 unit
+    spans more than 31 nonzero exponents above its base (the matrix must then stay in bf16)."""
+    _need_cuda(w)
+    if w.dtype != BF16 or w.dim() != 2 or w.stride(1) != 1:
+        raise ValueError("dlinear_pack: w must be a bf16 [N, K] matrix with unit column stride")
+    N, K = w.shape
+    buf = torch.empty(-(-N // 128) * (K // 64) * DLIN_PACKED_UNIT_BYTES, device=w.device, dtype=torch.uint8)
+    bad = torch.zeros(1, device=w.device, dtype=torch.int32)
+    _lib.check(_lib.load().u2_dlinear_pack_bf16(w.data_ptr(), N, K, w.stride(0), buf.data_ptr(), bad.data_ptr(),
+                                                _stream()), "u2_dlinear_pack_bf16")
+    return PackedWeight(buf, N, K) if int(bad.item()) == 0 else None
+
+
+def _dlinear_w(w):
+    """(data pointer, N, K, ldw, U2_DLIN_W_*) of a bf16 tensor or a PackedWeight."""
+    if isinstance(w, PackedWeight):
+        _need_cuda(w.buf)
+        return w.buf.data_ptr(), w.N, w.K, w.K, DLIN_W_PACKED13
+    _need_cuda(w)
+    return w.data_ptr(), w.shape[0], w.shape[1], w.stride(0), DLIN_W_BF16
+
+
 def _dlinear_desc(x, w, out, *, ws, counters, ssq_in=None, eps=1e-6, residual=None, silu_pair=False, gamma_next=None,
                   xg=None, ssq_out=None, ssq_zero=None, pdl=True, dbg=None, sched=0, dep_flags=None, dep_shift=1,
                   out_flags=None):
-    _need_cuda(x, w, out, ws, counters, ssq_in, residual, gamma_next, xg, ssq_out, ssq_zero)
+    _need_cuda(x, out, ws, counters, ssq_in, residual, gamma_next, xg, ssq_out, ssq_zero)
     d = _lib.DlinearDesc()
-    d.B, d.N, d.K = x.shape[0], w.shape[0], w.shape[1]
+    _, d.N, d.K, d.ldw, d.w_format = _dlinear_w(w)
+    d.B = x.shape[0]
     if counters.numel() < (d.N + 63) // 64 + (ssq_out is not None):
         raise ValueError("dlinear counters too small: ceil(N / 64) int32, + 1 with ssq_out")
     d.ws_elems = ws.numel()
-    d.ldx, d.ldw, d.ldy = x.stride(0), w.stride(0), out.stride(0)
+    d.ldx, d.ldy = x.stride(0), out.stride(0)
     d.ldr = residual.stride(0) if residual is not None else 0
     d.ldxg = xg.stride(0) if xg is not None else 0
     d.y_dtype = DT_BF16 if out.dtype == BF16 else DT_F32
@@ -444,32 +484,32 @@ def dlinear_new_ws(n_elems: int, device="cuda", lead=()) -> torch.Tensor:
     return torch.full((*lead, max(int(n_elems), 4)), -1, device=device, dtype=torch.int32).view(F32)
 
 
-def dlinear(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor, **kw):
-    """Decode-step linear on wgmma (see u2_dlinear_desc): x [B<=16, K] bf16, w [N, K] bf16."""
+def dlinear(x: torch.Tensor, w, out: torch.Tensor, **kw):
+    """Decode-step linear on wgmma (see u2_dlinear_desc): x [B<=16, K] bf16, w [N, K] bf16 or its PackedWeight."""
     d = _dlinear_desc(x, w, out, **kw)
-    _lib.check(_lib.load().u2_dlinear_bf16(x.data_ptr(), w.data_ptr(), out.data_ptr(), C.byref(d), _stream()),
+    _lib.check(_lib.load().u2_dlinear_bf16(x.data_ptr(), _dlinear_w(w)[0], out.data_ptr(), C.byref(d), _stream()),
                "u2_dlinear_bf16")
     return out
 
 
 def dlinear_multi(ops_list, *, gridbar: torch.Tensor, step_dev: torch.Tensor, pdl: bool = True,
                   lookahead_units: int = 0, next_weights=(), pre_stages: int = 0):
-    """Several dependent decode linears in ONE launch. ops_list: [(x, w, out, kwargs), ...] (max 4).
-    next_weights: [(w, units_per_cta), ...] (max 2) to warm L2 for the next launch."""
+    """Several dependent decode linears in ONE launch. ops_list: [(x, w, out, kwargs), ...] (max 4); the weights are
+    either all bf16 or all PackedWeight. next_weights: [(w, units_per_cta), ...] (max 2) to warm L2 for the next launch."""
     n = len(ops_list)
     descs = (_lib.DlinearDesc * n)()
     xs, ws_, ys = (C.c_void_p * n)(), (C.c_void_p * n)(), (C.c_void_p * n)()
     for i, (x, w, out, kw) in enumerate(ops_list):
         descs[i] = _dlinear_desc(x, w, out, **kw)
-        xs[i], ws_[i], ys[i] = x.data_ptr(), w.data_ptr(), out.data_ptr()
+        xs[i], ws_[i], ys[i] = x.data_ptr(), _dlinear_w(w)[0], out.data_ptr()
     _need_cuda(gridbar, step_dev)
     nx = _lib.DlinearNext()
     nx.lookahead_units = lookahead_units
     nx.pre_stages = pre_stages
     nx.n = len(next_weights)
     for j, (wn, units) in enumerate(next_weights):
-        _need_cuda(wn)
-        nx.w[j], nx.N[j], nx.K[j], nx.ldw[j], nx.units[j] = wn.data_ptr(), wn.shape[0], wn.shape[1], wn.stride(0), units
+        nx.w[j], nx.N[j], nx.K[j], nx.ldw[j], nx.w_format[j] = _dlinear_w(wn)
+        nx.units[j] = units
     _lib.check(_lib.load().u2_dlinear_multi_bf16(xs, ws_, ys, descs, n, gridbar.data_ptr(), step_dev.data_ptr(),
                                                  int(pdl), C.byref(nx), _stream()), "u2_dlinear_multi_bf16")
 
