@@ -459,6 +459,42 @@ U2_API int u2_logits_process_f32(float* logits, int32_t B, int32_t V, int64_t ld
                                  int64_t ld_hist, int32_t hist_cap, const u2_logits_proc_params* params_dev,
                                  const int32_t* step_dev, int32_t step, void* stream);
 
+/* Continuous batching (generate_batch): every row of the decode batch is a slot that holds one sample of one request,
+ * admitted and retired independently of the other rows. The per-slot state lives in DEVICE memory, one record per row,
+ * so one captured decode step serves every request that passes through the slots:
+ *   seed     the request's sampling seed;
+ *   row      the RNG row: j for the request's j-th sample (num_return_sequences);
+ *   count    tokens generated so far = the request's own step (what *step_dev is for a request decoded alone);
+ *   max_new  the request's max_new_tokens;
+ *   done     0: decoding; 1: finished or never admitted (the slot feeds pad and keeps its cache length).
+ * u2_sample_slots_f32 and u2_logits_process_slots_f32 are u2_sample_dev_f32 / u2_logits_process_f32 with the seed,
+ * the RNG row and the step (history length) of row b read from slots[b]: a slot draws and processes exactly what its
+ * request would draw and process alone. u2_slot_update runs after the pick: for every slot with done == 0 it stores
+ * ids[b] at out[b * ld_out + count] (when count < ld_out), increments count, and sets done on an EOS id of
+ * params_dev->eos or on count == max_new; a slot that goes on advances length[b] and length_plus1[b] (both optional).
+ * Every done slot gets ids[b] = params_dev->pad. */
+typedef struct u2_slot_state {
+  uint64_t seed;
+  int32_t row;
+  int32_t count;
+  int32_t max_new;
+  int32_t done;
+} u2_slot_state;
+typedef struct u2_slot_params {
+  int64_t pad;
+  int32_t n_eos;     /* <= U2_LP_MAX_EOS */
+  int32_t eos[U2_LP_MAX_EOS];
+  int32_t reserved;
+} u2_slot_params;
+U2_API int u2_sample_slots_f32(const float* logits, int64_t* out, int32_t B, int32_t V, int64_t ld,
+                               const u2_sample_params* params_dev, const u2_slot_state* slots, void* stream);
+U2_API int u2_logits_process_slots_f32(float* logits, int32_t B, int32_t V, int64_t ld, const int64_t* ids,
+                                       int32_t* hist, int64_t ld_hist, int32_t hist_cap,
+                                       const u2_logits_proc_params* params_dev, const u2_slot_state* slots,
+                                       void* stream);
+U2_API int u2_slot_update(int64_t* ids, int32_t B, u2_slot_state* slots, int64_t* out, int64_t ld_out,
+                          const u2_slot_params* params_dev, int32_t* length, int32_t* length_plus1, void* stream);
+
 /* Beam search (HF generate(num_beams=K, length_penalty, early_stopping): GenerationMixin._beam_search, transformers
  * generation/utils.py, with the prompt length 0 of generate(inputs_embeds=...)) inside the captured decode step.
  * Prompt b owns rows b*K .. b*K+K-1 of the decode batch; row b*K+k is HF's running beam k. One step:

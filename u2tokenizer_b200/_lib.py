@@ -222,6 +222,17 @@ class LogitsProcParams(C.Structure):
     ]
 
 
+class SlotState(C.Structure):
+    """Mirror of ``u2_slot_state`` (one record per decode row, in device memory)."""
+    _fields_ = [("seed", C.c_uint64), ("row", C.c_int32), ("count", C.c_int32), ("max_new", C.c_int32),
+                ("done", C.c_int32)]
+
+
+class SlotParams(C.Structure):
+    """Mirror of ``u2_slot_params`` (copied to device memory as raw bytes)."""
+    _fields_ = [("pad", C.c_int64), ("n_eos", C.c_int32), ("eos", C.c_int32 * LP_MAX_EOS), ("reserved", C.c_int32)]
+
+
 BEAM_MAX_BEAMS, BEAM_MAX_EOS, BEAM_MAX_KEEP = 16, 8, 144  # U2_BEAM_MAX_* of include/u2b200.h
 
 
@@ -286,6 +297,9 @@ SIGNATURES = {
     "u2_sample_f32": (C.c_int, [_P, _P, _I, _I, _L, _F, _I, _F, C.c_uint64, _P, _I, _P]),
     "u2_sample_dev_f32": (C.c_int, [_P, _P, _I, _I, _L, _P, _P, _I, _P]),
     "u2_logits_process_f32": (C.c_int, [_P, _I, _I, _L, _P, _P, _L, _I, _P, _P, _I, _P]),
+    "u2_sample_slots_f32": (C.c_int, [_P, _P, _I, _I, _L, _P, _P, _P]),
+    "u2_logits_process_slots_f32": (C.c_int, [_P, _I, _I, _L, _P, _P, _L, _I, _P, _P, _P]),
+    "u2_slot_update": (C.c_int, [_P, _I, _P, _P, _L, _P, _P, _P, _P]),
     "u2_topk_rows_f32": (C.c_int, [_P, _P, _I, _I, _I, _L, _L, _P]),
     "u2_log_softmax_f32": (C.c_int, [_P, _P, _I, _I, _L, _L, _P]),
     "u2_beam_topk_f32": (C.c_int, [_P, _L, _I, _I, _P, _P, _P, _P, _P, _P]),

@@ -18,12 +18,13 @@ constexpr int kLpThreads = 1024;
 __global__ void __launch_bounds__(kLpThreads)
 logits_process_kernel(float* __restrict__ logits, long long ld, int V, const long long* __restrict__ ids,
                       int* __restrict__ hist, long long ldh, int hist_cap, const u2_logits_proc_params* __restrict__ p,
-                      const int* __restrict__ step_dev, int step_host) {
+                      const int* __restrict__ step_dev, int step_host, const u2_slot_state* __restrict__ slots) {
   extern __shared__ unsigned int s_seen[];  // one bit per vocabulary entry
   const int b = blockIdx.x;
   float* l = logits + (long long)b * ld;
   int* h = hist + (long long)b * ldh;
-  const int t = min(step_dev ? *step_dev : step_host, hist_cap);  // history length
+  // history length; continuous batching: the slot's own generated count
+  const int t = min(slots ? slots[b].count : step_dev ? *step_dev : step_host, hist_cap);
   const int cur = t > 0 ? (int)ids[b] : 0;
   if (threadIdx.x == 0 && t > 0) h[t - 1] = cur;
   // slot t - 1 is read from `cur`, never from memory thread 0 is writing
@@ -102,10 +103,9 @@ logits_process_kernel(float* __restrict__ logits, long long ld, int V, const lon
 
 }  // namespace u2
 
-extern "C" U2_API int u2_logits_process_f32(float* logits, int32_t B, int32_t V, int64_t ld, const int64_t* ids,
-                                            int32_t* hist, int64_t ld_hist, int32_t hist_cap,
-                                            const u2_logits_proc_params* params_dev, const int32_t* step_dev,
-                                            int32_t step, void* stream) {
+static int logits_process_launch(float* logits, int32_t B, int32_t V, int64_t ld, const int64_t* ids, int32_t* hist,
+                                 int64_t ld_hist, int32_t hist_cap, const u2_logits_proc_params* params_dev,
+                                 const int32_t* step_dev, int32_t step, const u2_slot_state* slots, void* stream) {
   using namespace u2;
   if (!logits || !ids || !hist || !params_dev) return set_error(U2_ERR_ARG, "logits_process: null pointer");
   if (B <= 0 || V <= 0) return U2_OK;
@@ -118,7 +118,23 @@ extern "C" U2_API int u2_logits_process_f32(float* logits, int32_t B, int32_t V,
     if (e != cudaSuccess) return set_error(U2_ERR_CUDA, "logits_process: cudaFuncSetAttribute failed");
   }
   logits_process_kernel<<<B, kLpThreads, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
-      logits, ld, V, reinterpret_cast<const long long*>(ids), hist, ld_hist, hist_cap, params_dev, step_dev, step);
+      logits, ld, V, reinterpret_cast<const long long*>(ids), hist, ld_hist, hist_cap, params_dev, step_dev, step, slots);
   U2_CHECK_LAUNCH("logits_process");
   return U2_OK;
+}
+
+extern "C" U2_API int u2_logits_process_f32(float* logits, int32_t B, int32_t V, int64_t ld, const int64_t* ids,
+                                            int32_t* hist, int64_t ld_hist, int32_t hist_cap,
+                                            const u2_logits_proc_params* params_dev, const int32_t* step_dev,
+                                            int32_t step, void* stream) {
+  return logits_process_launch(logits, B, V, ld, ids, hist, ld_hist, hist_cap, params_dev, step_dev, step, nullptr,
+                               stream);
+}
+
+extern "C" U2_API int u2_logits_process_slots_f32(float* logits, int32_t B, int32_t V, int64_t ld, const int64_t* ids,
+                                                  int32_t* hist, int64_t ld_hist, int32_t hist_cap,
+                                                  const u2_logits_proc_params* params_dev, const u2_slot_state* slots,
+                                                  void* stream) {
+  if (!slots) return u2::set_error(U2_ERR_ARG, "logits_process_slots: null pointer");
+  return logits_process_launch(logits, B, V, ld, ids, hist, ld_hist, hist_cap, params_dev, nullptr, 0, slots, stream);
 }

@@ -48,7 +48,7 @@ __device__ __forceinline__ unsigned int mix32(unsigned int x) {
 __global__ void __launch_bounds__(kSampThreads)
 sample_kernel(const float* __restrict__ logits, long long ld, int V, float inv_temp, int top_k, float top_p,
               unsigned long long seed, const u2_sample_params* __restrict__ pdev, const int* __restrict__ step_dev,
-              int step_host, long long* __restrict__ out) {
+              int step_host, const u2_slot_state* __restrict__ slots, long long* __restrict__ out) {
   __shared__ float red[kSampThreads / 32];
   __shared__ float s_scan[kSampThreads];
   if (pdev) {
@@ -59,6 +59,7 @@ sample_kernel(const float* __restrict__ logits, long long ld, int V, float inv_t
     seed = pdev->seed;
   }
   const int b = blockIdx.x;
+  if (slots) seed = slots[b].seed;  // continuous batching: the slot's request keys its own stream
   const float* l = logits + (long long)b * ld;
   const int tid = threadIdx.x;
   // contiguous chunk per thread (index order matters for the final walk)
@@ -114,9 +115,10 @@ sample_kernel(const float* __restrict__ logits, long long ld, int V, float inv_t
   s_scan[tid] = mine;
   __syncthreads();
   if (tid == 0) {
-    const int step = step_dev ? *step_dev : step_host;
+    const int step = slots ? slots[b].count : step_dev ? *step_dev : step_host;
+    const int row = slots ? slots[b].row : b;
     unsigned int h = mix32((unsigned int)seed ^ mix32((unsigned int)(seed >> 32) + 0x9e3779b9u * (unsigned int)(step + 1)));
-    h = mix32(h ^ (0x85ebca6bu * (unsigned int)(b + 1)));
+    h = mix32(h ^ (0x85ebca6bu * (unsigned int)(row + 1)));
     const float u = ((h >> 8) + 0.5f) * (1.0f / 16777216.0f);  // (0,1)
     float total = 0.f;
     for (int t = 0; t < kSampThreads; ++t) total += s_scan[t];
@@ -155,7 +157,8 @@ extern "C" U2_API int u2_sample_f32(const float* logits, int64_t* out, int32_t B
   if (!(temperature > 0.f)) return set_error(U2_ERR_ARG, "sample: temperature must be > 0");
   if (!(top_p > 0.f) || top_p > 1.f) return set_error(U2_ERR_ARG, "sample: top_p must be in (0, 1]");
   sample_kernel<<<B, kSampThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      logits, ld, V, 1.0f / temperature, top_k, top_p, seed, nullptr, step_dev, step, reinterpret_cast<long long*>(out));
+      logits, ld, V, 1.0f / temperature, top_k, top_p, seed, nullptr, step_dev, step, nullptr,
+      reinterpret_cast<long long*>(out));
   U2_CHECK_LAUNCH("sample");
   return U2_OK;
 }
@@ -167,7 +170,18 @@ extern "C" U2_API int u2_sample_dev_f32(const float* logits, int64_t* out, int32
   if (!logits || !out || !params_dev) return set_error(U2_ERR_ARG, "sample_dev: null pointer");
   if (B <= 0 || V <= 0) return U2_OK;
   sample_kernel<<<B, kSampThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      logits, ld, V, 1.0f, 0, 1.0f, 0ull, params_dev, step_dev, step, reinterpret_cast<long long*>(out));
+      logits, ld, V, 1.0f, 0, 1.0f, 0ull, params_dev, step_dev, step, nullptr, reinterpret_cast<long long*>(out));
   U2_CHECK_LAUNCH("sample_dev");
+  return U2_OK;
+}
+
+extern "C" U2_API int u2_sample_slots_f32(const float* logits, int64_t* out, int32_t B, int32_t V, int64_t ld,
+                                          const u2_sample_params* params_dev, const u2_slot_state* slots, void* stream) {
+  using namespace u2;
+  if (!logits || !out || !params_dev || !slots) return set_error(U2_ERR_ARG, "sample_slots: null pointer");
+  if (B <= 0 || V <= 0) return U2_OK;
+  sample_kernel<<<B, kSampThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      logits, ld, V, 1.0f, 0, 1.0f, 0ull, params_dev, nullptr, 0, slots, reinterpret_cast<long long*>(out));
+  U2_CHECK_LAUNCH("sample_slots");
   return U2_OK;
 }

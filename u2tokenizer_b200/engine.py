@@ -19,7 +19,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import asdict, dataclass, replace
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, Iterable, List, Optional, Tuple
 
 import torch
 
@@ -755,7 +755,8 @@ class U2Engine:
         tc_rows = 16
         return tc_rows if self._use_tc_decode(tc_rows) else 8
 
-    def decode_step_tc(self, cache: "KVCache", req: Optional[GenerateRequest] = None) -> torch.Tensor:
+    def decode_step_tc(self, cache: "KVCache", req: Optional[GenerateRequest] = None,
+                       slots: Optional[dict] = None) -> torch.Tensor:
         """Decode step with every linear on the wgmma stream-K kernel and the RMSNorms folded into its
         epilogues. Launches per step: embed, qkv(0), then per layer [fused attention, one multi-op launch
         o_proj -> gate|up -> down -> next qkv (or lm_head)], argmax  =  2 launches per layer."""
@@ -810,9 +811,37 @@ class U2Engine:
             else:
                 for (xi, wi, yi, kw) in chain:
                     ops.dlinear(xi, wi, yi, pdl=self.pdl, **kw)
-        self._pick_next(logits, ids.view(B), bufs["step"], req)
-        cache.advance_device()
+        self._pick_or_slot_pick(logits, ids.view(B), bufs["step"], req, cache, slots)
         return logits
+
+    def _pick_or_slot_pick(self, logits, ids_out, step_dev, req, cache: "KVCache", slots: Optional[dict]):
+        """The end of a decode step: the pick and cache.advance_device(), or with `slots` (a continuous-batching state)
+        the per-slot pick and slot bookkeeping of _slot_pick."""
+        if slots is None:
+            self._pick_next(logits, ids_out, step_dev, req)
+            cache.advance_device()
+        else:
+            self._slot_pick(logits, ids_out, slots, req, cache)
+
+    def _slot_pick(self, logits: torch.Tensor, ids_out: torch.Tensor, st: dict, req: GenerateRequest,
+                   cache: Optional["KVCache"] = None):
+        """The token-picking head of continuous batching: _pick_next with the seed, RNG row and step (history length) of
+        every row read from its slot record st['slots'], so each slot picks what its request would pick decoded alone;
+        then ops.slot_update appends the picks to st['out'], finishes slots on EOS / max_new_tokens, feeds st['pad'] to
+        finished slots and advances the cache lengths of the others. cache None: an admission's first pick, from the
+        prefill logits (the host sets its lengths)."""
+        if req.processors is not None:
+            blk = self._param_block("logits processors", ops.logits_proc_params, self.g.vocab_size,
+                                    **asdict(req.processors))
+            ops.logits_process_slots(logits, blk, ids_out, st["hist"], st["slots"])
+        if req.sampling is None:
+            ops.argmax(logits, ids_out)
+        else:
+            ops.sample_slots(logits, self._param_block("sampling parameters", ops.sample_params, *req.sampling),
+                             st["slots"], ids_out)
+        ops.slot_update(ids_out, st["slots"], st["out"],
+                        self._param_block("slot parameters", ops.slot_params, st["pad"], req.eos_token_id),
+                        None if cache is None else cache.length_dev, None if cache is None else cache.length_plus1_dev)
 
     def _pick_next(self, logits: torch.Tensor, ids_out: torch.Tensor, step_dev: Optional[torch.Tensor],
                    req: Optional[GenerateRequest], step: int = 0):
@@ -870,14 +899,16 @@ class U2Engine:
         ops.beam_step(blk, bs, ids_out, st["cache"].kv_src, st["cache"].length_dev, V=logits.shape[1],
                       hist=st.get("hist"), step=step, step_dev=step_dev)
 
-    def decode_step(self, cache: "KVCache", req: Optional[GenerateRequest] = None) -> torch.Tensor:
+    def decode_step(self, cache: "KVCache", req: Optional[GenerateRequest] = None,
+                    slots: Optional[dict] = None) -> torch.Tensor:
         """Consumes buffers['ids'] [B,1] (the last token of every sequence), appends sequence b to the cache at
         position cache.length_dev[b] (read on the device), leaves fp32 logits in buffers['logits'] and the next ids
-        back in buffers['ids'], picked as `req` asks (None: greedy argmax). Launch sequence is CUDA-graph capturable."""
+        back in buffers['ids'], picked as `req` asks (None: greedy argmax). Launch sequence is CUDA-graph capturable.
+        slots: the state of a continuous-batching call (_SlotDecoder), whose rows pick per slot (_slot_pick)."""
         g = self.g
         B = cache.batch
         if self._use_tc_decode(B):
-            return self.decode_step_tc(cache, req)
+            return self.decode_step_tc(cache, req, slots)
         hq, hkv, dh = g.num_attention_heads, g.num_key_value_heads, g.head_dim
         bufs = self._decode_buffers(B)
         x, qkv, ctx, act, logits, ids = (bufs[k] for k in ("x", "qkv", "ctx", "act", "logits", "ids"))
@@ -896,8 +927,7 @@ class U2Engine:
             ops.gemv(act, w["wdown"], x, residual=x)
         ops.gemv(x, self.lm_head, logits, norm_gamma=self.final_norm, norm_eps=g.rms_norm_eps)
         bufs["step"] += 1  # the gemv path has no decode_embed kernel to bump the step counter
-        self._pick_next(logits, ids.view(B), bufs["step"], req)
-        cache.advance_device()
+        self._pick_or_slot_pick(logits, ids.view(B), bufs["step"], req, cache, slots)
         return logits
 
     # =========================================================================================
@@ -1009,20 +1039,24 @@ class U2Engine:
             outs = [torch.nn.functional.pad(o, (0, width - o.shape[1]), value=eos[0]) for o in outs]
         return torch.cat(outs, dim=0)
 
-    def _gen_state_for(self, B: int, cap: int, req: GenerateRequest):
+    def _gen_state_for(self, B: int, cap: int, req: GenerateRequest, slot_width: int = 0):
         """The static KV cache and the captured decode-step graph are kept across calls with the same (batch, capacity,
         head configuration): capture + instantiation cost ~0.1 s, which would otherwise be paid per request. With logits
         processors the state also holds the history of generated tokens, int32 [B, cap]; with beam search (K > 1) the
-        cache's indirection table and the beam buffers of ops.beam_step."""
+        cache's indirection table and the beam buffers of ops.beam_step. slot_width > 0 (continuous batching): the slot
+        records (ops.slot_state) and the generated tokens of every slot, int64 [B, slot_width]."""
         K = req.beam.num_beams if req.beam is not None else 1
         key = (B, cap, self.decode_impl, self.multi_op, self.fine_deps, req.sampling is not None,
-               req.processors is not None, K)
+               req.processors is not None, K, slot_width)
         st = self._gen_state if (self._gen_state is not None and self._gen_state["key"] == key) else None
         if st is None:
             self._gen_state = None  # drop the old cache before allocating the new one
             st = dict(key=key, cache=self.new_cache(B, cap), graph=None)
             if req.processors is not None:
                 st["hist"] = torch.zeros(B, cap, device=self.dev, dtype=torch.int32)
+            if slot_width:
+                st["slots"] = torch.zeros(B, ops.SLOT_STATE_BYTES, device=self.dev, dtype=torch.uint8)
+                st["out"] = torch.zeros(B, slot_width, device=self.dev, dtype=torch.int64)
             if K > 1:
                 st["cache"].kv_src = torch.zeros(B, cap, device=self.dev, dtype=torch.int32)
                 i32 = dict(device=self.dev, dtype=torch.int32)
@@ -1142,6 +1176,220 @@ class U2Engine:
                 bufs["ids"].view(B).copy_(force_ids[:, step])
             n_done += 1
         return out[:, :n_done]
+
+    # =========================================================================================
+    # continuous batching: finished decode rows are refilled with queued requests between graph replays
+    # =========================================================================================
+    @torch.no_grad()
+    def generate_continuous(self, requests: Iterable["SlotRequest"], num_slots: int, eos_token_id=None,
+                            pad_token_id: int = 0, do_sample: bool = False, temperature: float = 1.0, top_k: int = 50,
+                            top_p: float = 1.0, num_return_sequences: int = 1,
+                            processors: Optional[LogitsProcessors] = None,
+                            use_graph: bool = True) -> Dict[str, List[List[int]]]:
+        """Decodes every request of `requests` (read lazily) through num_slots decode rows; each request's n =
+        num_return_sequences samples take n rows, admitted together as soon as n rows are free. Every row generates
+        what generate() gives for its request alone: the same prefill, and a pick keyed by the request's seed, the
+        sample's index and the request's own step. Returns {request_id: n token lists}, each up to and including the
+        first EOS. Statistics of the call: last_continuous (steps, captures, admissions)."""
+        cap = self._decode_rows()
+        if not 1 <= num_slots <= cap:
+            raise ValueError(f"num_slots={num_slots} outside 1..{cap} (the rows one decode step carries on this path)")
+        if not 1 <= num_return_sequences <= num_slots:
+            raise ValueError(f"num_return_sequences={num_return_sequences} outside 1..num_slots={num_slots}")
+        sampling = (float(temperature), int(top_k or 0), float(top_p), 0) if do_sample else None
+        req = GenerateRequest(0, eos_token_id, sampling, processors)  # max_new_tokens and the seed live in the slots
+        dec = _SlotDecoder(self, req, num_slots, int(pad_token_id), use_graph)
+        sched = SlotScheduler(dec, num_slots, num_return_sequences)
+        out = sched.run(requests)
+        self.last_continuous = dict(steps=sched.steps, captures=dec.captures, admissions=sched.admissions,
+                                    capacity=sched.capacity)
+        return out
+
+
+SLOT_POLL_STEPS = 8  # decode steps between two polls of the slots' done flags (DESIGN.md, continuous batching)
+SLOT_CAP_ROUND = 128
+
+
+def slot_capacity(max_prompt: int, max_new_tokens: int) -> int:
+    """KV capacity of a continuous-batching cache: the longest prompt admitted so far, rounded up to a multiple of 128,
+    plus the largest max_new_tokens (a row's last decode step writes position prompt + max_new_tokens - 2)."""
+    return -(-max_prompt // SLOT_CAP_ROUND) * SLOT_CAP_ROUND + max_new_tokens
+
+
+@dataclass
+class SlotRequest:
+    """One request of a continuous-batching call as the engine takes it: the prompt's embeddings [1, L, E] (bf16, on the
+    device; what generate() prefills for it alone), its own max_new_tokens and sampling seed."""
+    request_id: str
+    embeds: Optional[torch.Tensor]
+    max_new_tokens: int
+    seed: int = 0
+
+    @property
+    def prompt_len(self) -> int:
+        return int(self.embeds.shape[1])
+
+
+class SlotScheduler:
+    """The host policy of continuous batching, over a backend that owns the device state (_SlotDecoder on the GPU):
+      reserve(capacity, width)  make the cache hold `capacity` positions and `width` tokens per slot, keeping the live
+                                slots (called before the first admission and whenever a request needs more);
+      admit(request, slots)     prefill the request and start its n samples in the given slots;
+      step()                    one decode step over every slot;
+      snapshot() / read(h)      enqueue a copy of the slots' state without waiting; read it back (waits for the copy):
+                                per slot its generated tokens when it is finished, else None.
+    Free slots are taken lowest first. A request is pulled from the iterable only when a slot is free, and waits for n
+    free slots. Every SLOT_POLL_STEPS steps the snapshot taken SLOT_POLL_STEPS steps earlier is read and a new one is
+    enqueued: the host never waits on the step it just queued, so the device keeps the queued steps to run while the
+    host retires and admits."""
+
+    def __init__(self, backend, num_slots: int, samples: int = 1):
+        self.b, self.S, self.n = backend, num_slots, samples
+        self.steps = self.admissions = self.capacity = 0
+
+    def run(self, requests) -> Dict[str, List[List[int]]]:
+        it = iter(requests)
+        free, owner = list(range(self.S)), [None] * self.S
+        parts, results = {}, {}
+        pending, exhausted, snap = None, False, None
+        max_len = max_new = 0
+        while True:
+            while True:
+                if pending is None:
+                    if exhausted or not free:
+                        break
+                    pending = next(it, None)
+                    if pending is None:
+                        exhausted = True
+                        break
+                    if pending.request_id in parts or pending.request_id in results:
+                        raise ValueError(f"duplicate request_id {pending.request_id!r}")
+                    if pending.max_new_tokens < 1:
+                        raise ValueError(f"request {pending.request_id!r}: max_new_tokens must be >= 1")
+                if len(free) < self.n:
+                    break
+                slots, free = free[:self.n], free[self.n:]
+                max_len, max_new = max(max_len, pending.prompt_len), max(max_new, pending.max_new_tokens)
+                need = slot_capacity(max_len, max_new)
+                if need > self.capacity:
+                    self.b.reserve(need, max_new)
+                    self.capacity = need
+                self.b.admit(pending, slots)
+                self.admissions += 1
+                parts[pending.request_id] = [None] * self.n
+                for j, s in enumerate(slots):
+                    owner[s] = (pending.request_id, j)
+                pending = None
+            if all(o is None for o in owner):
+                return results
+            self.b.step()
+            self.steps += 1
+            if self.steps % SLOT_POLL_STEPS == 0:
+                if snap is not None:
+                    handle, owners_then = snap
+                    for s, toks in enumerate(self.b.read(handle)):
+                        # a slot refilled after the snapshot was taken shows its previous request's state: skip it
+                        if toks is None or owner[s] is None or owner[s] != owners_then[s]:
+                            continue
+                        rid, j = owner[s]
+                        parts[rid][j] = toks
+                        owner[s] = None
+                        free.append(s)
+                        if all(p is not None for p in parts[rid]):
+                            results[rid] = parts.pop(rid)
+                    free.sort()
+                snap = (self.b.snapshot(), list(owner))
+
+
+class _SlotDecoder:
+    """The device side of SlotScheduler on a U2Engine: a static cache of num_slots rows with their slot records, and
+    one captured decode step (decode_step with slots) per (slots, capacity). Admissions, polls and cache growth run on
+    the decode stream, between replays."""
+
+    def __init__(self, eng: U2Engine, req: GenerateRequest, num_slots: int, pad: int, use_graph: bool):
+        self.eng, self.req, self.S, self.pad, self.use_graph = eng, req, num_slots, pad, use_graph
+        self.st, self.captures = None, 0
+        eng.reset_decode_state(num_slots)
+        self.ids = eng._decode_buffers(num_slots)["ids"].view(num_slots)
+
+    def reserve(self, capacity: int, width: int):
+        old, eng = self.st, self.eng
+        st = eng._gen_state_for(self.S, capacity, self.req, slot_width=width)
+        st["pad"] = self.pad
+        if old is None:
+            # no slot holds a request yet: every record is done (pad fed, lengths frozen at 0)
+            st["slots"].copy_(ops.slot_state([0] * self.S, [0] * self.S, [1] * self.S, done=[1] * self.S))
+            st["cache"].set_length(0)
+        else:
+            # a longer prompt or max_new_tokens arrived: the live slots move to the larger cache
+            T0, w0 = old["cache"].max_len, old["out"].shape[1]
+            for a, b in ((st["cache"].k, old["cache"].k), (st["cache"].v, old["cache"].v)):
+                a[:, :, :, :T0].copy_(b)
+            for name in ("length_dev", "length_plus1_dev"):
+                getattr(st["cache"], name).copy_(getattr(old["cache"], name))
+            st["slots"].copy_(old["slots"])
+            st["out"][:, :w0].copy_(old["out"])
+            if "hist" in st:
+                st["hist"][:, :T0].copy_(old["hist"])
+        self.st = st
+
+    def admit(self, r: SlotRequest, slots: List[int]):
+        """generate()'s batch-1 prefill of the request, its KV rows copied into each of its slots (as the n > 1 path
+        of _generate copies them), and the first pick from the prefill logits with the request's own (seed, row) head."""
+        eng, st, n = self.eng, self.st, len(slots)
+        L = r.prompt_len
+        pc = eng.new_cache(1, L)
+        hidden = eng.prefill(r.embeds, pc)
+        logits0 = eng.lm_logits(eng._last_hidden(hidden, torch.tensor([L])))
+        logits0 = logits0.index_select(0, torch.zeros(n, dtype=torch.int64, device=eng.dev))
+        first = dict(slots=ops.slot_state([r.seed] * n, range(n), [r.max_new_tokens] * n).to(eng.dev),
+                     out=torch.empty(n, 1, device=eng.dev, dtype=torch.int64), pad=self.pad)
+        if "hist" in st:
+            first["hist"] = torch.zeros(n, 1, device=eng.dev, dtype=torch.int32)  # count 0: no history is read
+        ids = torch.empty(n, device=eng.dev, dtype=torch.int64)
+        eng._slot_pick(logits0, ids, first, self.req)
+        cache = st["cache"]
+        for s in slots:
+            cache.k[:, s, :, :L].copy_(pc.k[:, 0])
+            cache.v[:, s, :, :L].copy_(pc.v[:, 0])
+        idx = torch.tensor(slots, device=eng.dev)
+        cache.length_dev.index_fill_(0, idx, L)
+        cache.length_plus1_dev.index_fill_(0, idx, L + 1)
+        st["slots"].index_copy_(0, idx, first["slots"])
+        st["out"][:, 0].index_copy_(0, idx, first["out"][:, 0])
+        self.ids.index_copy_(0, idx, ids)
+        if "hist" in st:
+            st["hist"].index_fill_(0, idx, 0)
+
+    def step(self):
+        st = self.st
+        run = lambda: self.eng.decode_step(st["cache"], self.req, slots=st)
+        if not self.use_graph or not st.get("warm"):
+            run()  # the first step on a new state runs eagerly (it also configures the kernels' attributes)
+            st["warm"] = True
+            return
+        if st["graph"] is None:
+            self.captures += 1
+        self.eng._replay(st, run)
+
+    def snapshot(self):
+        st = self.st
+        recs = torch.empty(st["slots"].shape, dtype=torch.uint8, pin_memory=True)
+        out = torch.empty(st["out"].shape, dtype=torch.int64, pin_memory=True)
+        recs.copy_(st["slots"], non_blocking=True)
+        out.copy_(st["out"], non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        return ev, recs, out
+
+    @staticmethod
+    def read(handle) -> List[Optional[List[int]]]:
+        ev, recs, out = handle
+        ev.synchronize()
+        f = ops.slot_state_fields(recs)
+        return [out[s, :c].tolist() if d else None
+                for s, (c, d) in enumerate(zip(f["count"].tolist(), f["done"].tolist()))]
+
 
 class KVCache:
     """Static KV cache [layers][B, Hkv, Tmax, dh] bf16 + the current length of every sequence on the device

@@ -16,6 +16,7 @@ Running them without CUDA / without libu2b200.so raises - there is no PyTorch fa
 from __future__ import annotations
 
 from abc import ABC, abstractmethod
+from dataclasses import dataclass
 from typing import Any, Dict, List, Optional, Tuple, Union
 
 import numpy as np
@@ -165,6 +166,19 @@ class U2MetaModel:
             w = torch.load(model_args.pretrain_mm_mlp_adapter, map_location="cpu")
             self.mm_projector.load_state_dict({k.split("mm_projector.")[1]: v for k, v in w.items() if "mm_projector" in k},
                                               strict=True)
+
+
+@dataclass
+class GenerationOutput:
+    """One request's result from generate_batch(), with the field names of HF's continuous-batching output.
+    generated_tokens: the new token ids up to and including the first EOS (what generate() returns for the request's
+    row before it pads); with num_return_sequences = n > 1, a list of n such lists, sample 0 first."""
+    request_id: str
+    prompt_ids: List[int]
+    generated_tokens: list
+
+
+_BATCH_REQUEST_KEYS = ("images", "input_ids", "question_ids", "max_new_tokens", "seed", "request_id")
 
 
 class U2MetaForCausalLM(ABC):
@@ -552,6 +566,134 @@ class U2MetaForCausalLM(ABC):
             keep = int((~after).any(dim=0).sum())
             ids = ids[:, :max(keep, 1)]
         return ids  # new tokens only, like HF generate() on inputs_embeds (reference u2llama.py:123-127)
+
+    @torch.no_grad()
+    def generate_batch(self, requests, num_slots: Optional[int] = None, **kwargs) -> Dict[str, GenerationOutput]:
+        """Continuous batching over many studies: every request runs as if generate() ran it alone, but a decode row
+        whose request has finished is refilled with the next queued request instead of idling until its batch ends.
+        requests: any iterable of dicts with `images` ([1, C, D, H, W] or [C, D, H, W], CPU or CUDA), `input_ids` ([L]
+        or [1, L], unpadded) and optionally `question_ids`, `max_new_tokens`, `seed` and `request_id` (default: the
+        request's index as a string); it is read lazily, so only the requests in the decode rows are held.
+        num_slots: decode rows in flight (default and maximum: the rows one decode step carries, 16 on the wgmma path).
+        kwargs: generate()'s greedy / sampling / num_return_sequences / logits-processor / eos / pad options. Request i
+        without a seed samples with seed + i. Returns {request_id: GenerationOutput}."""
+        eng = self.engine()
+        gc = getattr(self, "generation_config", None)
+        head = self._generate_batch_head(kwargs, gc, num_slots, eng._decode_rows(), eng.g.vocab_size)
+        n_vis = eng.g.num_3d_query_token if eng.g.enable_u2tokenizer else eng.g.tokens_per_frame
+        prompts = {}
+
+        def engine_requests():
+            from .engine import SlotRequest
+            for i, r in enumerate(requests):
+                p = self._generate_batch_request(i, r, head["seed"])
+                ids, images = p["input_ids"], p["images"]
+                if images is not None and self.get_vision_tower() is not None and ids.shape[1] != 1:
+                    if ids.shape[1] < 1 + n_vis:
+                        raise ValueError(f"request {p['request_id']!r}: {ids.shape[1]} prompt tokens, at least "
+                                         f"{1 + n_vis} needed (<bos> + the visual tokens)")
+                    emb = eng.multimodal_embeds(ids, images, p["question_ids"])
+                else:
+                    emb = eng.embed_tokens(ids)
+                max_new = p["max_new_tokens"]
+                if max_new is None:
+                    max_new = head["max_new_tokens"]
+                if max_new is None:  # max_length counts the prompt, as in generate()
+                    max_new = max(1, head["max_length"] - ids.shape[1])
+                prompts[p["request_id"]] = ids[0].tolist()
+                yield SlotRequest(p["request_id"], emb.to(torch.bfloat16), int(max_new), p["seed"])
+
+        out = eng.generate_continuous(engine_requests(), head["num_slots"], eos_token_id=head["eos"],
+                                      pad_token_id=head["pad"], do_sample=head["do_sample"],
+                                      temperature=head["temperature"], top_k=head["top_k"], top_p=head["top_p"],
+                                      num_return_sequences=head["n"], processors=head["processors"])
+        return {rid: GenerationOutput(rid, prompts[rid], seqs[0] if head["n"] == 1 else seqs)
+                for rid, seqs in out.items()}
+
+    def _generate_batch_head(self, kwargs: dict, gc, num_slots, rows: int, vocab_size: int) -> dict:
+        """generate_batch()'s options, read and validated by generate()'s helpers and generation_config fallbacks."""
+        from .engine import eos_ids
+        num_beams = kwargs.pop("num_beams", None)
+        if num_beams is None:
+            num_beams = getattr(gc, "num_beams", None) or 1
+        if num_beams != 1:
+            raise NotImplementedError("generate_batch() does not run beam search (num_beams > 1); use generate()")
+        do_sample = kwargs.pop("do_sample", None)
+        if do_sample is None:
+            do_sample = bool(getattr(gc, "do_sample", False))
+
+        def opt(name, default):
+            v = kwargs.pop(name, None)
+            if v is None and gc is not None:
+                v = getattr(gc, name, None)
+            return default if v is None else v
+        temperature, top_k, top_p = opt("temperature", 1.0), opt("top_k", 50), opt("top_p", 1.0)
+        seed = kwargs.pop("seed", None)
+        if seed is None:
+            seed = int(torch.initial_seed()) + self.__dict__.setdefault("_u2_sample_calls", 0)
+            self.__dict__["_u2_sample_calls"] += 1
+        max_new = kwargs.pop("max_new_tokens", None)
+        max_length = kwargs.pop("max_length", None) or getattr(gc, "max_length", None) or 20
+        eos = kwargs.pop("eos_token_id", None)
+        eos = eos_ids(gc.eos_token_id if eos is None and gc is not None else eos)
+        pad = kwargs.pop("pad_token_id", None)
+        if pad is None and gc is not None:
+            pad = gc.pad_token_id
+        if pad is not None and not isinstance(pad, (int, np.integer)):
+            pad = int(torch.as_tensor(pad).reshape(-1)[0])
+        n_ret = int(opt("num_return_sequences", 1))
+        min_new_set = kwargs.get("min_new_tokens") is not None or getattr(gc, "min_new_tokens", None) is not None
+        if not min_new_set and (kwargs.get("min_length") or getattr(gc, "min_length", None) or 0) > 0:
+            raise NotImplementedError("generate_batch(): min_length counts each prompt's width; pass min_new_tokens")
+        procs = self._generate_logits_processors(kwargs, gc, 0, eos, vocab_size)
+        self._check_remaining_generate_kwargs(kwargs)
+        if n_ret > 1 and not do_sample:
+            raise ValueError("num_return_sequences > 1 needs do_sample=True (greedy decoding is deterministic; HF raises too)")
+        S = rows if num_slots is None else num_slots
+        if isinstance(S, bool) or not isinstance(S, (int, np.integer)) or not 1 <= S <= rows:
+            raise ValueError(f"num_slots={num_slots!r} outside 1..{rows} (the rows one decode step carries)")
+        if not 1 <= n_ret <= S:
+            raise ValueError(f"num_return_sequences={n_ret} outside 1..num_slots={S}")
+        if len(eos) > _lib.LP_MAX_EOS:
+            raise ValueError(f"generate_batch() supports at most {_lib.LP_MAX_EOS} EOS ids, got {len(eos)}")
+        return dict(num_slots=int(S), n=n_ret, do_sample=bool(do_sample), temperature=temperature, top_k=top_k,
+                    top_p=top_p, seed=int(seed), max_new_tokens=max_new, max_length=int(max_length), eos=eos,
+                    pad=int(pad) if pad is not None else (eos[0] if eos else 0), processors=procs)
+
+    @staticmethod
+    def _generate_batch_request(i: int, r, seed: int) -> dict:
+        """Request i of generate_batch() -> input_ids [1, L], images [1, C, D, H, W] or None, question_ids, its
+        max_new_tokens (None: the call's), its seed (default seed + i) and its id (default str(i))."""
+        if not isinstance(r, dict):
+            raise TypeError(f"generate_batch(): request {i} must be a dict, got {type(r).__name__}")
+        unknown = sorted(set(r) - set(_BATCH_REQUEST_KEYS))
+        if unknown:
+            raise TypeError(f"generate_batch(): request {i} has unsupported keys {unknown}")
+        if r.get("input_ids") is None:
+            raise TypeError(f"generate_batch(): request {i} needs input_ids")
+        ids = torch.as_tensor(r["input_ids"])
+        if ids.dim() == 1:
+            ids = ids[None]
+        if ids.dim() != 2 or ids.shape[0] != 1 or ids.shape[1] < 1:
+            raise ValueError(f"generate_batch(): request {i}: input_ids must be [L] or [1, L], got {tuple(ids.shape)}")
+        images = r.get("images")
+        if images is not None:
+            if images.dim() == 4:
+                images = images[None]
+            if images.dim() != 5 or images.shape[0] != 1:
+                raise ValueError(f"generate_batch(): request {i}: images must be [C, D, H, W] or [1, C, D, H, W], got "
+                                 f"{tuple(images.shape)}")
+        q = r.get("question_ids")
+        if q is not None:
+            q = torch.as_tensor(q)
+            q = q[None] if q.dim() == 1 else q
+        mn = r.get("max_new_tokens")
+        if mn is not None and (isinstance(mn, bool) or not isinstance(mn, (int, np.integer)) or mn < 1):
+            raise ValueError(f"generate_batch(): request {i}: max_new_tokens must be a positive integer, got {mn!r}")
+        s = r.get("seed")
+        rid = r.get("request_id")
+        return dict(input_ids=ids, images=images, question_ids=q, max_new_tokens=None if mn is None else int(mn),
+                    seed=int(seed) + i if s is None else int(s), request_id=str(i) if rid is None else str(rid))
 
     @staticmethod
     def _generate_beam_search(kwargs: dict, generation_config, num_beams, do_sample: bool, num_return_sequences: int,

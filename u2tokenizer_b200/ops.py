@@ -705,6 +705,108 @@ def logits_process(logits: torch.Tensor, params: torch.Tensor, ids: torch.Tensor
     return logits
 
 
+SLOT_STATE_BYTES = C.sizeof(_lib.SlotState)
+
+
+def slot_state(seeds, rows, max_new, counts=None, done=None) -> torch.Tensor:
+    """u2_slot_state records (include/u2b200.h) for len(seeds) decode rows, as a CPU uint8 tensor [rows, 24]: per row
+    the request's seed, its RNG row, its generated count (default 0), its max_new_tokens and its done flag (default 0)."""
+    n = len(seeds)
+    recs = (_lib.SlotState * n)()
+    for i in range(n):
+        recs[i].seed = int(seeds[i]) & ((1 << 64) - 1)
+        recs[i].row, recs[i].max_new = int(rows[i]), int(max_new[i])
+        recs[i].count = 0 if counts is None else int(counts[i])
+        recs[i].done = 0 if done is None else int(done[i])
+    return torch.frombuffer(bytearray(bytes(recs)), dtype=torch.uint8).view(n, SLOT_STATE_BYTES)
+
+
+def slot_state_fields(state: torch.Tensor) -> dict:
+    """The count / done / row / max_new columns of slot_state() records (any device), as int32 tensors [rows]."""
+    w = state.view(torch.int32).view(-1, SLOT_STATE_BYTES // 4)
+    return dict(row=w[:, 2], count=w[:, 3], max_new=w[:, 4], done=w[:, 5])
+
+
+def _check_slots(slots: torch.Tensor, B: int):
+    if slots.dtype != torch.uint8 or tuple(slots.shape) != (B, SLOT_STATE_BYTES) or not slots.is_contiguous():
+        raise ValueError(f"slots must be the contiguous uint8 [{B}, {SLOT_STATE_BYTES}] records of slot_state()")
+
+
+def slot_params(device, pad_token_id: int, eos_token_ids=(), out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The u2_slot_params block (include/u2b200.h) in device memory, as uint8: the id a finished slot feeds and the EOS
+    ids that finish a slot. `out` (a block made earlier) is overwritten in place, as for sample_params()."""
+    eos = [int(e) for e in eos_token_ids]
+    if len(eos) > _lib.LP_MAX_EOS:
+        raise ValueError(f"at most {_lib.LP_MAX_EOS} EOS ids, got {len(eos)}")
+    blk = _lib.SlotParams()
+    blk.pad, blk.n_eos = int(pad_token_id), len(eos)
+    for i, e in enumerate(eos):
+        blk.eos[i] = e
+    host = torch.frombuffer(bytearray(bytes(blk)), dtype=torch.uint8)
+    if out is None:
+        return host.to(device)
+    out.copy_(host)
+    return out
+
+
+def sample_slots(logits: torch.Tensor, params: torch.Tensor, slots: torch.Tensor,
+                 out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """sample_dev() with the seed, RNG row and step of row b read from the slot record slots[b]."""
+    _need_cuda(logits, params, slots)
+    B, V = logits.shape
+    if params.dtype != torch.uint8 or params.numel() != 24:
+        raise ValueError("sample_slots: params must be the 24-byte block of sample_params()")
+    _check_slots(slots, B)
+    if out is None:
+        out = torch.empty(B, device=logits.device, dtype=torch.int64)
+    _lib.check(_lib.load().u2_sample_slots_f32(logits.data_ptr(), out.data_ptr(), B, V, logits.stride(0),
+                                               params.data_ptr(), slots.data_ptr(), _stream()), "u2_sample_slots_f32")
+    return out
+
+
+def logits_process_slots(logits: torch.Tensor, params: torch.Tensor, ids: torch.Tensor, hist: torch.Tensor,
+                         slots: torch.Tensor) -> torch.Tensor:
+    """logits_process() with the history length of row b read from the slot record slots[b] (its generated count)."""
+    _need_cuda(logits, params, ids, hist, slots)
+    B, V = logits.shape
+    if logits.dtype != F32 or logits.stride(1) != 1:
+        raise TypeError("logits_process_slots: logits must be fp32 with unit column stride")
+    if params.dtype != torch.uint8 or params.numel() != C.sizeof(_lib.LogitsProcParams):
+        raise ValueError("logits_process_slots: params must be the block of logits_proc_params()")
+    if ids.dtype != torch.int64 or ids.numel() != B or not ids.is_contiguous():
+        raise ValueError("logits_process_slots: ids must be contiguous int64 [B]")
+    if hist.dtype != torch.int32 or hist.dim() != 2 or hist.shape[0] != B or hist.stride(1) != 1:
+        raise ValueError("logits_process_slots: hist must be int32 [B, cap] with unit column stride")
+    _check_slots(slots, B)
+    _lib.check(_lib.load().u2_logits_process_slots_f32(logits.data_ptr(), B, V, logits.stride(0), ids.data_ptr(),
+                                                       hist.data_ptr(), hist.stride(0), hist.shape[1],
+                                                       params.data_ptr(), slots.data_ptr(), _stream()),
+               "u2_logits_process_slots_f32")
+    return logits
+
+
+def slot_update(ids: torch.Tensor, slots: torch.Tensor, out: torch.Tensor, params: torch.Tensor,
+                length: Optional[torch.Tensor] = None, length_plus1: Optional[torch.Tensor] = None) -> None:
+    """Slot bookkeeping after a pick (u2_slot_update): every decoding slot appends ids[b] to out[b] at its count,
+    counts it, finishes on an EOS id or max_new_tokens and, when the cache lengths are given, advances them; every
+    finished slot gets ids[b] = pad. ids int64 [B] (contiguous), out int64 [B, width], params: slot_params()."""
+    _need_cuda(ids, slots, out, params, length, length_plus1)
+    B = ids.numel()
+    if ids.dtype != torch.int64 or not ids.is_contiguous():
+        raise ValueError("slot_update: ids must be contiguous int64 [B]")
+    _check_slots(slots, B)
+    if out.dtype != torch.int64 or out.dim() != 2 or out.shape[0] != B or out.stride(1) != 1:
+        raise ValueError("slot_update: out must be int64 [B, width] with unit column stride")
+    if params.dtype != torch.uint8 or params.numel() != C.sizeof(_lib.SlotParams):
+        raise ValueError("slot_update: params must be the block of slot_params()")
+    for t in (length, length_plus1):
+        if t is not None and (t.dtype != torch.int32 or t.numel() != B or not t.is_contiguous()):
+            raise ValueError("slot_update: length / length_plus1 must be contiguous int32 [B]")
+    _lib.check(_lib.load().u2_slot_update(ids.data_ptr(), B, slots.data_ptr(), out.data_ptr(), out.stride(0),
+                                          params.data_ptr(), _ptr(length), _ptr(length_plus1), _stream()),
+               "u2_slot_update")
+
+
 def log_softmax(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Row-wise log_softmax of fp32 [rows, V] into `out` (a separate fp32 buffer)."""
     _need_cuda(x, out)
