@@ -495,6 +495,38 @@ U2_API int u2_logits_process_slots_f32(float* logits, int32_t B, int32_t V, int6
 U2_API int u2_slot_update(int64_t* ids, int32_t B, u2_slot_state* slots, int64_t* out, int64_t ld_out,
                           const u2_slot_params* params_dev, int32_t* length, int32_t* length_plus1, void* stream);
 
+/* Generation scores (HF generate(return_dict_in_generate, output_scores, output_logits) and continuous batching's
+ * return_logprobs), written inside the captured decode step. A feature that is off launches none of these.
+ * u2_row_store_params: the destination of a step-indexed row store, in DEVICE memory so that one captured step serves
+ * every call and chunk (the host rewrites the block before the first, eager, step of each chunk). Row r of step t is
+ * stored at dst + t * ld_step + r * ld_row; a step outside [0, steps) is not stored.
+ *   u2_store_rows_f32    copies src [rows, V] (row stride ld_src) to the rows of step t = *step_dev (or step when
+ *                        step_dev is NULL): the raw logits, greedy scores and beam scores of that step.
+ *   u2_sample_out_f32    u2_sample_dev_f32 (step from step_dev / step) or u2_sample_slots_f32 (slots not NULL; then
+ *                        step_dev must be NULL) with the same draw, bit for bit, that also writes, when not NULL,
+ *                        scores_dev's row: x * (1 / temperature) where the top-k / top-p cut keeps it, -inf elsewhere
+ *                        (what HF's warpers hand the multinomial), and logprob[b] = log softmax of that row at the pick.
+ *   u2_pick_logprob_f32  logprob[b] = logits[b, ids[b]] - logsumexp(logits[b]) (the greedy pick's log-prob).
+ *   u2_slot_update_lp    u2_slot_update that also stores lp_in[b] at lp_out[b * ld_out + count] for every live slot. */
+typedef struct u2_row_store_params {
+  float* dst;
+  int64_t ld_step;
+  int64_t ld_row;
+  int32_t steps;
+  int32_t reserved;
+} u2_row_store_params;
+U2_API int u2_store_rows_f32(const float* src, int32_t rows, int32_t V, int64_t ld_src,
+                             const u2_row_store_params* params_dev, const int32_t* step_dev, int32_t step, void* stream);
+U2_API int u2_sample_out_f32(const float* logits, int64_t* out, int32_t B, int32_t V, int64_t ld,
+                             const u2_sample_params* params_dev, const int32_t* step_dev, int32_t step,
+                             const u2_slot_state* slots, const u2_row_store_params* scores_dev, float* logprob,
+                             void* stream);
+U2_API int u2_pick_logprob_f32(const float* logits, int32_t B, int32_t V, int64_t ld, const int64_t* ids,
+                               float* logprob, void* stream);
+U2_API int u2_slot_update_lp(int64_t* ids, int32_t B, u2_slot_state* slots, int64_t* out, int64_t ld_out,
+                             const float* lp_in, float* lp_out, const u2_slot_params* params_dev, int32_t* length,
+                             int32_t* length_plus1, void* stream);
+
 /* Beam search (HF generate(num_beams=K, length_penalty, early_stopping): GenerationMixin._beam_search, transformers
  * generation/utils.py, with the prompt length 0 of generate(inputs_embeds=...)) inside the captured decode step.
  * Prompt b owns rows b*K .. b*K+K-1 of the decode batch; row b*K+k is HF's running beam k. One step:

@@ -233,6 +233,12 @@ class SlotParams(C.Structure):
     _fields_ = [("pad", C.c_int64), ("n_eos", C.c_int32), ("eos", C.c_int32 * LP_MAX_EOS), ("reserved", C.c_int32)]
 
 
+class RowStoreParams(C.Structure):
+    """Mirror of ``u2_row_store_params`` (copied to device memory as raw bytes)."""
+    _fields_ = [("dst", C.c_void_p), ("ld_step", C.c_int64), ("ld_row", C.c_int64), ("steps", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 BEAM_MAX_BEAMS, BEAM_MAX_EOS, BEAM_MAX_KEEP = 16, 8, 144  # U2_BEAM_MAX_* of include/u2b200.h
 
 
@@ -300,6 +306,10 @@ SIGNATURES = {
     "u2_sample_slots_f32": (C.c_int, [_P, _P, _I, _I, _L, _P, _P, _P]),
     "u2_logits_process_slots_f32": (C.c_int, [_P, _I, _I, _L, _P, _P, _L, _I, _P, _P, _P]),
     "u2_slot_update": (C.c_int, [_P, _I, _P, _P, _L, _P, _P, _P, _P]),
+    "u2_store_rows_f32": (C.c_int, [_P, _I, _I, _L, _P, _P, _I, _P]),
+    "u2_sample_out_f32": (C.c_int, [_P, _P, _I, _I, _L, _P, _P, _I, _P, _P, _P, _P]),
+    "u2_pick_logprob_f32": (C.c_int, [_P, _I, _I, _L, _P, _P, _P]),
+    "u2_slot_update_lp": (C.c_int, [_P, _I, _P, _P, _L, _P, _P, _P, _P, _P, _P]),
     "u2_topk_rows_f32": (C.c_int, [_P, _P, _I, _I, _I, _L, _L, _P]),
     "u2_log_softmax_f32": (C.c_int, [_P, _P, _I, _I, _L, _L, _P]),
     "u2_beam_topk_f32": (C.c_int, [_P, _L, _I, _I, _P, _P, _P, _P, _P, _P]),

@@ -224,6 +224,60 @@ __global__ void argmax_final_kernel(unsigned long long* __restrict__ scratch, lo
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Generation scores inside the captured decode step. A captured graph keeps its pointers, so the destination of a
+// step's row store is read from a device block (u2_row_store_params) and the step from *step_dev: one capture serves
+// every step, chunk and call. Grid (slices, rows); each CTA copies one slice of a row, coalesced.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+store_rows_kernel(const float* __restrict__ src, long long ld_src, int V, const u2_row_store_params* __restrict__ p,
+                  const int* __restrict__ step_dev, int step_host) {
+  const long long t = step_dev ? *step_dev : step_host;
+  if (t < 0 || t >= p->steps) return;
+  const int r = blockIdx.y;
+  const float* s = src + r * ld_src;
+  float* d = p->dst + t * p->ld_step + r * p->ld_row;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < V; i += gridDim.x * blockDim.x) d[i] = s[i];
+}
+
+// logprob[b] = logits[b, ids[b]] - logsumexp(logits[b]): one CTA per row, an online (max, sum of exp) per thread
+// merged across the block. Rows may hold -inf entries (logits processors); a row that is all -inf yields NaN.
+__global__ void __launch_bounds__(512)
+pick_logprob_kernel(const float* __restrict__ logits, long long ld, int V, const long long* __restrict__ ids,
+                    float* __restrict__ logprob) {
+  const int b = blockIdx.x;
+  const float* l = logits + b * ld;
+  float m = -INFINITY, s = 0.f;
+  for (int i = threadIdx.x; i < V; i += blockDim.x) {
+    const float x = l[i];
+    if (x > m) {
+      s = s * expf(m - x) + 1.f;
+      m = x;
+    } else if (x > -INFINITY) {
+      s += expf(x - m);
+    }
+  }
+  __shared__ float sm[16], ss[16];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+    const float mm = fmaxf(m, m2);
+    s = (m == -INFINITY ? 0.f : s * expf(m - mm)) + (m2 == -INFINITY ? 0.f : s2 * expf(m2 - mm));
+    m = mm;
+  }
+  if ((threadIdx.x & 31) == 0) { sm[threadIdx.x >> 5] = m; ss[threadIdx.x >> 5] = s; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float M = -INFINITY, S = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) {
+      const float mm = fmaxf(M, sm[w]);
+      S = (M == -INFINITY ? 0.f : S * expf(M - mm)) + (sm[w] == -INFINITY ? 0.f : ss[w] * expf(sm[w] - mm));
+      M = mm;
+    }
+    logprob[b] = (l[ids[b]] - M) - logf(S);
+  }
+}
+
 template <int kB>
 static int launch_gemv(const GemvArgs& a, cudaStream_t st) {
   const int n_out = a.silu_pair ? a.N / 2 : a.N;
@@ -290,5 +344,29 @@ extern "C" U2_API int u2_argmax_f32(const float* logits, int64_t* out, uint64_t*
   U2_CHECK_LAUNCH("argmax partial");
   argmax_final_kernel<<<1, 1024, 0, st>>>(reinterpret_cast<unsigned long long*>(scratch), reinterpret_cast<long long*>(out), B);
   U2_CHECK_LAUNCH("argmax final");
+  return U2_OK;
+}
+
+extern "C" U2_API int u2_store_rows_f32(const float* src, int32_t rows, int32_t V, int64_t ld_src,
+                                        const u2_row_store_params* params_dev, const int32_t* step_dev, int32_t step,
+                                        void* stream) {
+  if (!src || !params_dev) return set_error(U2_ERR_ARG, "store_rows: null pointer");
+  if (rows <= 0 || V <= 0) return U2_OK;
+  if (rows > 65535) return set_error(U2_ERR_UNSUPPORTED, "store_rows: rows <= 65535");
+  int slices = (V + 4095) / 4096;
+  if (slices > 64) slices = 64;
+  store_rows_kernel<<<dim3((unsigned)slices, (unsigned)rows), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      src, ld_src, V, params_dev, step_dev, step);
+  U2_CHECK_LAUNCH("store_rows");
+  return U2_OK;
+}
+
+extern "C" U2_API int u2_pick_logprob_f32(const float* logits, int32_t B, int32_t V, int64_t ld, const int64_t* ids,
+                                          float* logprob, void* stream) {
+  if (!logits || !ids || !logprob) return set_error(U2_ERR_ARG, "pick_logprob: null pointer");
+  if (B <= 0 || V <= 0) return U2_OK;
+  pick_logprob_kernel<<<B, 512, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      logits, ld, V, reinterpret_cast<const long long*>(ids), logprob);
+  U2_CHECK_LAUNCH("pick_logprob");
   return U2_OK;
 }

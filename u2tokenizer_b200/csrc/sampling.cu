@@ -45,10 +45,15 @@ __device__ __forceinline__ unsigned int mix32(unsigned int x) {
   return x;
 }
 
+// kOut: also write the warped scores row (x * inv_temp where kept, -inf elsewhere) into the step-indexed row store
+// `scores` (when not null) and the pick's log-prob under the kept distribution into logprob[b] (when not null). The
+// draw is the same code in both instantiations, so the ids are bit-identical.
+template <bool kOut>
 __global__ void __launch_bounds__(kSampThreads)
 sample_kernel(const float* __restrict__ logits, long long ld, int V, float inv_temp, int top_k, float top_p,
               unsigned long long seed, const u2_sample_params* __restrict__ pdev, const int* __restrict__ step_dev,
-              int step_host, const u2_slot_state* __restrict__ slots, long long* __restrict__ out) {
+              int step_host, const u2_slot_state* __restrict__ slots, long long* __restrict__ out,
+              const u2_row_store_params* __restrict__ scores = nullptr, float* __restrict__ logprob = nullptr) {
   __shared__ float red[kSampThreads / 32];
   __shared__ float s_scan[kSampThreads];
   if (pdev) {
@@ -106,6 +111,17 @@ sample_kernel(const float* __restrict__ logits, long long ld, int V, float inv_t
     }
     cut = lo;
   }
+  if constexpr (kOut) {
+    // the warped row, in index-strided order so that a warp's stores are coalesced (the row is L2-resident)
+    const long long t = slots ? slots[b].count : step_dev ? *step_dev : step_host;
+    if (scores && t >= 0 && t < scores->steps) {
+      float* srow = scores->dst + t * scores->ld_step + b * scores->ld_row;
+      for (int i = tid; i < V; i += kSampThreads) {
+        const float x = l[i] * inv_temp;
+        srow[i] = x >= cut ? x : -INFINITY;
+      }
+    }
+  }
   // ---- draw: u * kept mass, then locate it in index order
   float mine = 0.f;
   for (int i = i0; i < i1; ++i) {
@@ -143,6 +159,9 @@ sample_kernel(const float* __restrict__ logits, long long ld, int V, float inv_t
     }
     if (pick < 0) pick = last_kept >= 0 ? last_kept : 0;
     out[b] = pick;
+    if constexpr (kOut) {
+      if (logprob) logprob[b] = (l[pick] * inv_temp - mx) - logf(total);
+    }
   }
 }
 
@@ -156,7 +175,7 @@ extern "C" U2_API int u2_sample_f32(const float* logits, int64_t* out, int32_t B
   if (B <= 0 || V <= 0) return U2_OK;
   if (!(temperature > 0.f)) return set_error(U2_ERR_ARG, "sample: temperature must be > 0");
   if (!(top_p > 0.f) || top_p > 1.f) return set_error(U2_ERR_ARG, "sample: top_p must be in (0, 1]");
-  sample_kernel<<<B, kSampThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  sample_kernel<false><<<B, kSampThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       logits, ld, V, 1.0f / temperature, top_k, top_p, seed, nullptr, step_dev, step, nullptr,
       reinterpret_cast<long long*>(out));
   U2_CHECK_LAUNCH("sample");
@@ -169,7 +188,7 @@ extern "C" U2_API int u2_sample_dev_f32(const float* logits, int64_t* out, int32
   using namespace u2;
   if (!logits || !out || !params_dev) return set_error(U2_ERR_ARG, "sample_dev: null pointer");
   if (B <= 0 || V <= 0) return U2_OK;
-  sample_kernel<<<B, kSampThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  sample_kernel<false><<<B, kSampThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       logits, ld, V, 1.0f, 0, 1.0f, 0ull, params_dev, step_dev, step, nullptr, reinterpret_cast<long long*>(out));
   U2_CHECK_LAUNCH("sample_dev");
   return U2_OK;
@@ -180,8 +199,23 @@ extern "C" U2_API int u2_sample_slots_f32(const float* logits, int64_t* out, int
   using namespace u2;
   if (!logits || !out || !params_dev || !slots) return set_error(U2_ERR_ARG, "sample_slots: null pointer");
   if (B <= 0 || V <= 0) return U2_OK;
-  sample_kernel<<<B, kSampThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  sample_kernel<false><<<B, kSampThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       logits, ld, V, 1.0f, 0, 1.0f, 0ull, params_dev, nullptr, 0, slots, reinterpret_cast<long long*>(out));
   U2_CHECK_LAUNCH("sample_slots");
+  return U2_OK;
+}
+
+extern "C" U2_API int u2_sample_out_f32(const float* logits, int64_t* out, int32_t B, int32_t V, int64_t ld,
+                                        const u2_sample_params* params_dev, const int32_t* step_dev, int32_t step,
+                                        const u2_slot_state* slots, const u2_row_store_params* scores_dev,
+                                        float* logprob, void* stream) {
+  using namespace u2;
+  if (!logits || !out || !params_dev) return set_error(U2_ERR_ARG, "sample_out: null pointer");
+  if (slots && step_dev) return set_error(U2_ERR_ARG, "sample_out: the step comes from slots or step_dev, not both");
+  if (B <= 0 || V <= 0) return U2_OK;
+  sample_kernel<true><<<B, kSampThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      logits, ld, V, 1.0f, 0, 1.0f, 0ull, params_dev, step_dev, step, slots, reinterpret_cast<long long*>(out),
+      scores_dev, logprob);
+  U2_CHECK_LAUNCH("sample_out");
   return U2_OK;
 }

@@ -81,12 +81,18 @@ class GenerateRequest:
     """What the token-picking head of one generate() call does, handed to every decode step of the call.
     sampling: (temperature, top_k, top_p, seed), or None for greedy argmax. processors: a neutral configuration is kept
     as None, so it runs exactly as no configuration: no extra launch, the same captured graph. beam: num_beams > 1, or
-    None; with it the sampling is ignored. eos_token_id: anything eos_ids() takes, kept as its tuple."""
+    None; with it the sampling is ignored. eos_token_id: anything eos_ids() takes, kept as its tuple.
+    output_scores / output_logits: every step also stores the scores the token was picked from / the raw logits into
+    the row stores set by _set_row_store() (HF generate(output_scores, output_logits)). return_logprobs (continuous
+    batching): every slot also records the log-prob of each pick. All three off: exactly the launches without them."""
     max_new_tokens: int
     eos_token_id: Tuple[int, ...] = ()
     sampling: Optional[Tuple[float, int, float, int]] = None
     processors: Optional[LogitsProcessors] = None
     beam: Optional[BeamSearch] = None
+    output_scores: bool = False
+    output_logits: bool = False
+    return_logprobs: bool = False
 
     def __post_init__(self):
         object.__setattr__(self, "eos_token_id", eos_ids(self.eos_token_id))
@@ -834,21 +840,31 @@ class U2Engine:
             blk = self._param_block("logits processors", ops.logits_proc_params, self.g.vocab_size,
                                     **asdict(req.processors))
             ops.logits_process_slots(logits, blk, ids_out, st["hist"], st["slots"])
+        lp = (st["lp_step"], st["lp"]) if req.return_logprobs else None
         if req.sampling is None:
             ops.argmax(logits, ids_out)
+            if lp is not None:
+                ops.pick_logprob(logits, ids_out, lp[0])
         else:
-            ops.sample_slots(logits, self._param_block("sampling parameters", ops.sample_params, *req.sampling),
-                             st["slots"], ids_out)
+            params = self._param_block("sampling parameters", ops.sample_params, *req.sampling)
+            if lp is not None:
+                ops.sample_out(logits, params, ids_out, logprob=lp[0], slots=st["slots"])
+            else:
+                ops.sample_slots(logits, params, st["slots"], ids_out)
         ops.slot_update(ids_out, st["slots"], st["out"],
                         self._param_block("slot parameters", ops.slot_params, st["pad"], req.eos_token_id),
-                        None if cache is None else cache.length_dev, None if cache is None else cache.length_plus1_dev)
+                        None if cache is None else cache.length_dev, None if cache is None else cache.length_plus1_dev,
+                        lp=lp)
 
     def _pick_next(self, logits: torch.Tensor, ids_out: torch.Tensor, step_dev: Optional[torch.Tensor],
                    req: Optional[GenerateRequest], step: int = 0):
         """Greedy argmax (req None: plain argmax), or the sampled head (temperature -> top-k -> top-p -> multinomial)
         when the request samples (HF generate(do_sample=True, ...), reference eval/mrg.py:74-75). The request's logits
         processors rewrite the logits in place first, from the generation state's history of generated tokens.
-        Beam search replaces all of it with the beam step (_beam_pick)."""
+        Beam search replaces all of it with the beam step (_beam_pick). The requested outputs are stored at the step:
+        the raw logits before the processors, the scores (processed logits, or the sampler's warped row) after them."""
+        if req is not None and req.output_logits:
+            ops.store_rows(logits, self._row_store("logits"), step=step, step_dev=step_dev)
         if req is not None and req.beam is not None:
             return self._beam_pick(logits, ids_out, step_dev, req, step)
         if req is not None and req.processors is not None:
@@ -856,12 +872,25 @@ class U2Engine:
                                     **asdict(req.processors))
             ops.logits_process(logits, blk, ids_out, self._gen_state["hist"], step=step, step_dev=step_dev)
         if req is None or req.sampling is None:
+            if req is not None and req.output_scores:
+                ops.store_rows(logits, self._row_store("scores"), step=step, step_dev=step_dev)
             ops.argmax(logits, ids_out)
         else:
             # parameters (seed included) are read from a device block: the captured decode graph survives a new
             # request's seed / temperature / top-k / top-p
-            ops.sample_dev(logits, self._param_block("sampling parameters", ops.sample_params, *req.sampling), ids_out,
-                           step=step, step_dev=step_dev)
+            params = self._param_block("sampling parameters", ops.sample_params, *req.sampling)
+            if req.output_scores:
+                ops.sample_out(logits, params, ids_out, scores=self._row_store("scores"), step=step, step_dev=step_dev)
+            else:
+                ops.sample_dev(logits, params, ids_out, step=step, step_dev=step_dev)
+
+    def _set_row_store(self, what: str, dst: torch.Tensor) -> None:
+        """Points the `what` row store ("logits" or "scores") at dst, an fp32 [steps, rows, V] view: the decode steps of
+        the chunk that follows store step t's rows into dst[t]. Call it before the chunk's first (eager) pick."""
+        self._param_block(what + " store", ops.row_store_params, **ops.row_store_dst(dst))
+
+    def _row_store(self, what: str) -> torch.Tensor:
+        return self._param_blocks[what + " store"][1]
 
     def _param_block(self, what: str, make, *args, **kw) -> torch.Tensor:
         """The device block make(self.dev, *args, **kw) builds (ops.sample_params, logits_proc_params or beam_params),
@@ -895,6 +924,8 @@ class U2Engine:
             pblk = self._param_block("logits processors", ops.logits_proc_params, self.g.vocab_size,
                                      **asdict(req.processors))
             ops.logits_process(lp, pblk, ids_out, st["hist"], step=step, step_dev=step_dev)
+        if req.output_scores:
+            ops.store_rows(lp, self._row_store("scores"), step=step, step_dev=step_dev)
         ops.beam_topk(lp, bs["running"], bs["flags"], blk, bs["cand_val"], bs["cand_tok"])
         ops.beam_step(blk, bs, ids_out, st["cache"].kv_src, st["cache"].length_dev, V=logits.shape[1],
                       hist=st.get("hist"), step=step, step_dev=step_dev)
@@ -937,7 +968,7 @@ class U2Engine:
     def generate(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id=None, do_sample: bool = False,
                  temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, seed: int = 0, use_graph: bool = True,
                  num_return_sequences: int = 1, lengths=None, processors: Optional[LogitsProcessors] = None,
-                 beam: Optional[BeamSearch] = None):
+                 beam: Optional[BeamSearch] = None, output_scores: bool = False, output_logits: bool = False):
         """Greedy (do_sample=False) or sampled decoding; same loop, only the token-picking head differs.
         processors (optional): HF's repetition penalty / no-repeat n-gram / bad words / min new tokens, applied to every
         step's logits before the pick; every row of a chunk of rows keeps its own history of generated tokens.
@@ -947,13 +978,20 @@ class U2Engine:
         lengths [B] (optional): prompt b is embeds[b, :lengths[b]] (right padding after it); it decodes from position
         lengths[b] on, as if it ran alone. None = every prompt fills the whole width.
         beam (num_beams > 1): HF beam search instead of the greedy / sampled pick (do_sample and num_return_sequences are
-        then ignored; the beam config carries its own num_return_sequences)."""
+        then ignored; the beam config carries its own num_return_sequences).
+        output_scores / output_logits (HF generate's): the call returns (ids, scores, logits), each of the last two an fp32
+        [max_new_tokens, rows, V] tensor (or None when not asked) whose step t holds every row's scores (greedy: the
+        processed logits; sampled: the warped row, -inf where top-k / top-p dropped the token; beam: the processed
+        log-probs of all num_beams rows of every prompt) / raw logits. They cost max_new_tokens * rows * V * 4 bytes each,
+        allocated before decoding starts so that an out-of-memory error comes first; steps after a chunk of rows stopped
+        early (every row hit EOS) hold 0."""
         lens = self._row_lengths(lengths, embeds.shape[0], embeds.shape[1])
+        outputs = dict(output_scores=bool(output_scores), output_logits=bool(output_logits))
         if beam is not None and beam.num_beams > 1:
             return self._generate(embeds, GenerateRequest(max_new_tokens, eos_token_id, processors=processors,
-                                                          beam=beam), lens, use_graph)
+                                                          beam=beam, **outputs), lens, use_graph)
         sampling = (float(temperature), int(top_k or 0), float(top_p), int(seed)) if do_sample else None
-        req = GenerateRequest(max_new_tokens, eos_token_id, sampling, processors)
+        req = GenerateRequest(max_new_tokens, eos_token_id, sampling, processors, **outputs)
         return self._generate(embeds, req, lens, use_graph, max(1, int(num_return_sequences)))
 
     def generate_greedy(self, embeds: torch.Tensor, max_new_tokens: int, eos_token_id=None,
@@ -986,7 +1024,9 @@ class U2Engine:
         lens: the CPU prompt lengths of _row_lengths(). margins / force_ids / logits_out: the hooks of generate_greedy()
         (logits_out also receives the raw logits of a beam search), for a request that fits one chunk.
         Greedy and sampled chunks that stop early are padded to the common width with the first EOS id; beam search
-        returns n_ret hypotheses per prompt, best first, filled with HF's fill value (last_beam_scores: their scores)."""
+        returns n_ret hypotheses per prompt, best first, filled with HF's fill value (last_beam_scores: their scores,
+        last_beam_indices: HF's beam_indices). With req.output_scores / output_logits: (ids, scores, logits), see
+        generate()."""
         B, L, _ = embeds.shape
         cap, bm, eos = self._decode_rows(), req.beam, req.eos_token_id
         if bm is not None:
@@ -1002,10 +1042,15 @@ class U2Engine:
         plan = chunk_plan(B, n, cap, bm is not None)
         if len(plan) > 1 and (margins is not None or force_ids is not None or logits_out is not None):
             raise ValueError(f"return_margins / force_ids / logits_out need at most {cap} rows, got {B * n}")
+        stores = {}
+        for what, on in (("scores", req.output_scores), ("logits", req.output_logits)):
+            if on:  # steps x rows x V x 4 bytes, allocated before any decoding
+                stores[what] = torch.zeros(req.max_new_tokens, B * n, self.g.vocab_size, device=self.dev, dtype=F32)
         if n > 1:
             pc = self.new_cache(B, L)
             logits0 = self.lm_logits(self._last_hidden(self.prefill(embeds, pc), lens))
-        outs, seqs, scores = [], [], []
+        outs, seqs, scores, beam_idx = [], [], [], []
+        r0 = 0
         for src, seed_off in plan:
             r = req if req.sampling is None else replace(req, sampling=(*req.sampling[:3], req.sampling[3] + seed_off))
             st = self._gen_state_for(len(src), L + req.max_new_tokens, r)
@@ -1021,23 +1066,32 @@ class U2Engine:
                 hidden = self.prefill(embeds[int(src[0]):int(src[-1]) + 1], cache)
                 cache.set_length(lens[src])
                 chunk_logits0 = self.lm_logits(self._last_hidden(hidden, lens[src]))
+            for what, buf in stores.items():  # this chunk's rows of the caller's [steps, B * n, V]
+                self._set_row_store(what, buf[:, r0:r0 + len(src)])
             if bm is not None:
                 self._beam_loop(st, chunk_logits0, r, use_graph, logits_out)
-                s, sc = self._beam_backtrack(st["beam"], len(src) // K, K, n_ret, fill)
+                s, sc, bi = self._beam_backtrack(st["beam"], len(src) // K, K, n_ret, fill, row0=r0)
                 seqs += s
                 scores.append(sc)
+                beam_idx += bi
             else:
                 outs.append(self._decode_loop(st, chunk_logits0, r, use_graph, margins, force_ids, logits_out))
+            r0 += len(src)
+        extra = (stores.get("scores"), stores.get("logits")) if stores else ()
         if bm is not None:
             out = torch.full((len(seqs), max(len(x) for x in seqs)), fill, dtype=torch.int64)
-            for i, x in enumerate(seqs):
+            idx = torch.full(out.shape, -1, dtype=torch.int32)
+            for i, (x, b) in enumerate(zip(seqs, beam_idx)):
                 out[i, :len(x)] = torch.as_tensor(x, dtype=torch.int64)
+                idx[i, :len(b)] = torch.as_tensor(b, dtype=torch.int32)
             self.last_beam_scores = torch.cat(scores)
-            return out.to(self.dev)
+            self.last_beam_indices = idx.to(self.dev)
+            return (out.to(self.dev), *extra) if extra else out.to(self.dev)
         width = max(o.shape[1] for o in outs)
         if any(o.shape[1] != width for o in outs):  # chunks that hit EOS early: pad with EOS (masked by the caller)
             outs = [torch.nn.functional.pad(o, (0, width - o.shape[1]), value=eos[0]) for o in outs]
-        return torch.cat(outs, dim=0)
+        out = torch.cat(outs, dim=0)
+        return (out, *extra) if extra else out
 
     def _gen_state_for(self, B: int, cap: int, req: GenerateRequest, slot_width: int = 0):
         """The static KV cache and the captured decode-step graph are kept across calls with the same (batch, capacity,
@@ -1047,7 +1101,7 @@ class U2Engine:
         records (ops.slot_state) and the generated tokens of every slot, int64 [B, slot_width]."""
         K = req.beam.num_beams if req.beam is not None else 1
         key = (B, cap, self.decode_impl, self.multi_op, self.fine_deps, req.sampling is not None,
-               req.processors is not None, K, slot_width)
+               req.processors is not None, K, slot_width, req.output_scores, req.output_logits, req.return_logprobs)
         st = self._gen_state if (self._gen_state is not None and self._gen_state["key"] == key) else None
         if st is None:
             self._gen_state = None  # drop the old cache before allocating the new one
@@ -1057,6 +1111,9 @@ class U2Engine:
             if slot_width:
                 st["slots"] = torch.zeros(B, ops.SLOT_STATE_BYTES, device=self.dev, dtype=torch.uint8)
                 st["out"] = torch.zeros(B, slot_width, device=self.dev, dtype=torch.int64)
+                if req.return_logprobs:
+                    st["lp"] = torch.zeros(B, slot_width, device=self.dev, dtype=F32)
+                    st["lp_step"] = torch.zeros(B, device=self.dev, dtype=F32)
             if K > 1:
                 st["cache"].kv_src = torch.zeros(B, cap, device=self.dev, dtype=torch.int32)
                 i32 = dict(device=self.dev, dtype=torch.int32)
@@ -1114,25 +1171,30 @@ class U2Engine:
                 logits_out.append(bufs["logits"].clone())
 
     @staticmethod
-    def _beam_backtrack(bs: dict, P: int, K: int, n_ret: int, fill: int):
-        """The best n_ret finished hypotheses of every prompt, rebuilt from the per-step (token, parent beam) records."""
+    def _beam_backtrack(bs: dict, P: int, K: int, n_ret: int, fill: int, row0: int = 0):
+        """The best n_ret finished hypotheses of every prompt, rebuilt from the per-step (token, parent beam) records,
+        with their scores and HF's beam_indices: per step, the row (row0 + p * K + beam) the token was appended to."""
         info = bs["fin_info"].cpu().numpy()
         score = bs["fin_score"].cpu()
         rec = bs["rec"].cpu().numpy()
-        seqs, keep = [], []
+        seqs, keep, rows = [], [], []
         for p in range(P):
             for i in range(n_ret):
                 r = p * K + i
                 _, te, beam, tok = (int(x) for x in info[r])
                 seq = [fill] * (te + 1)
+                row = [-1] * (te + 1)
                 if te >= 0:
                     seq[te] = tok
+                    row[te] = row0 + p * K + beam
                     for s in range(te - 1, -1, -1):
                         seq[s] = int(rec[s, p * K + beam, 0])
                         beam = int(rec[s, p * K + beam, 1])
+                        row[s] = row0 + p * K + beam
                 seqs.append(seq)
                 keep.append(r)
-        return seqs, score[keep]
+                rows.append(row)
+        return seqs, score[keep], rows
 
     def _decode_loop(self, st, logits0: torch.Tensor, req: GenerateRequest, use_graph: bool,
                      margins: Optional[list] = None, force_ids: Optional[torch.Tensor] = None,
@@ -1184,20 +1246,23 @@ class U2Engine:
     def generate_continuous(self, requests: Iterable["SlotRequest"], num_slots: int, eos_token_id=None,
                             pad_token_id: int = 0, do_sample: bool = False, temperature: float = 1.0, top_k: int = 50,
                             top_p: float = 1.0, num_return_sequences: int = 1,
-                            processors: Optional[LogitsProcessors] = None,
-                            use_graph: bool = True) -> Dict[str, List[List[int]]]:
+                            processors: Optional[LogitsProcessors] = None, use_graph: bool = True,
+                            return_logprobs: bool = False) -> Dict[str, list]:
         """Decodes every request of `requests` (read lazily) through num_slots decode rows; each request's n =
         num_return_sequences samples take n rows, admitted together as soon as n rows are free. Every row generates
         what generate() gives for its request alone: the same prefill, and a pick keyed by the request's seed, the
         sample's index and the request's own step. Returns {request_id: n token lists}, each up to and including the
-        first EOS. Statistics of the call: last_continuous (steps, captures, admissions)."""
+        first EOS; with return_logprobs, n (tokens, log-probs) pairs instead, the log-prob of each token under the
+        distribution it was picked from (log_softmax of its scores). Statistics of the call: last_continuous (steps,
+        captures, admissions)."""
         cap = self._decode_rows()
         if not 1 <= num_slots <= cap:
             raise ValueError(f"num_slots={num_slots} outside 1..{cap} (the rows one decode step carries on this path)")
         if not 1 <= num_return_sequences <= num_slots:
             raise ValueError(f"num_return_sequences={num_return_sequences} outside 1..num_slots={num_slots}")
         sampling = (float(temperature), int(top_k or 0), float(top_p), 0) if do_sample else None
-        req = GenerateRequest(0, eos_token_id, sampling, processors)  # max_new_tokens and the seed live in the slots
+        # max_new_tokens and the seed live in the slots
+        req = GenerateRequest(0, eos_token_id, sampling, processors, return_logprobs=bool(return_logprobs))
         dec = _SlotDecoder(self, req, num_slots, int(pad_token_id), use_graph)
         sched = SlotScheduler(dec, num_slots, num_return_sequences)
         out = sched.run(requests)
@@ -1237,7 +1302,7 @@ class SlotScheduler:
       admit(request, slots)     prefill the request and start its n samples in the given slots;
       step()                    one decode step over every slot;
       snapshot() / read(h)      enqueue a copy of the slots' state without waiting; read it back (waits for the copy):
-                                per slot its generated tokens when it is finished, else None.
+                                per slot its result (its generated tokens) when it is finished, else None.
     Free slots are taken lowest first. A request is pulled from the iterable only when a slot is free, and waits for n
     free slots. Every SLOT_POLL_STEPS steps the snapshot taken SLOT_POLL_STEPS steps earlier is read and a new one is
     enqueued: the host never waits on the step it just queued, so the device keeps the queued steps to run while the
@@ -1329,6 +1394,8 @@ class _SlotDecoder:
                 getattr(st["cache"], name).copy_(getattr(old["cache"], name))
             st["slots"].copy_(old["slots"])
             st["out"][:, :w0].copy_(old["out"])
+            if "lp" in st:
+                st["lp"][:, :w0].copy_(old["lp"])
             if "hist" in st:
                 st["hist"][:, :T0].copy_(old["hist"])
         self.st = st
@@ -1346,6 +1413,9 @@ class _SlotDecoder:
                      out=torch.empty(n, 1, device=eng.dev, dtype=torch.int64), pad=self.pad)
         if "hist" in st:
             first["hist"] = torch.zeros(n, 1, device=eng.dev, dtype=torch.int32)  # count 0: no history is read
+        if "lp" in st:
+            first["lp"] = torch.empty(n, 1, device=eng.dev, dtype=F32)
+            first["lp_step"] = torch.empty(n, device=eng.dev, dtype=F32)
         ids = torch.empty(n, device=eng.dev, dtype=torch.int64)
         eng._slot_pick(logits0, ids, first, self.req)
         cache = st["cache"]
@@ -1357,6 +1427,8 @@ class _SlotDecoder:
         cache.length_plus1_dev.index_fill_(0, idx, L + 1)
         st["slots"].index_copy_(0, idx, first["slots"])
         st["out"][:, 0].index_copy_(0, idx, first["out"][:, 0])
+        if "lp" in st:
+            st["lp"][:, 0].index_copy_(0, idx, first["lp"][:, 0])
         self.ids.index_copy_(0, idx, ids)
         if "hist" in st:
             st["hist"].index_fill_(0, idx, 0)
@@ -1378,17 +1450,25 @@ class _SlotDecoder:
         out = torch.empty(st["out"].shape, dtype=torch.int64, pin_memory=True)
         recs.copy_(st["slots"], non_blocking=True)
         out.copy_(st["out"], non_blocking=True)
+        lp = None
+        if "lp" in st:
+            lp = torch.empty(st["lp"].shape, dtype=F32, pin_memory=True)
+            lp.copy_(st["lp"], non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
-        return ev, recs, out
+        return ev, recs, out, lp
 
     @staticmethod
-    def read(handle) -> List[Optional[List[int]]]:
-        ev, recs, out = handle
+    def read(handle) -> list:
+        """Per slot its tokens, or (tokens, log-probs) with return_logprobs, when it is finished; else None."""
+        ev, recs, out, lp = handle
         ev.synchronize()
         f = ops.slot_state_fields(recs)
-        return [out[s, :c].tolist() if d else None
-                for s, (c, d) in enumerate(zip(f["count"].tolist(), f["done"].tolist()))]
+        done = [(s, c) for s, (c, d) in enumerate(zip(f["count"].tolist(), f["done"].tolist())) if d]
+        res = [None] * out.shape[0]
+        for s, c in done:
+            res[s] = out[s, :c].tolist() if lp is None else (out[s, :c].tolist(), lp[s, :c].tolist())
+        return res
 
 
 class KVCache:

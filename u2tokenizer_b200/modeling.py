@@ -16,7 +16,7 @@ Running them without CUDA / without libu2b200.so raises - there is no PyTorch fa
 from __future__ import annotations
 
 from abc import ABC, abstractmethod
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from typing import Any, Dict, List, Optional, Tuple, Union
 
 import numpy as np
@@ -24,6 +24,7 @@ import torch
 import torch.nn as nn
 from transformers import (AutoConfig, AutoModelForCausalLM, LlamaForCausalLM, LlamaModel, Phi3ForCausalLM, Phi3Model,
                           Qwen3ForCausalLM, Qwen3Model)
+from transformers.generation import GenerateBeamDecoderOnlyOutput, GenerateDecoderOnlyOutput
 from transformers.modeling_outputs import CausalLMOutputWithPast
 
 from . import _lib
@@ -172,10 +173,13 @@ class U2MetaModel:
 class GenerationOutput:
     """One request's result from generate_batch(), with the field names of HF's continuous-batching output.
     generated_tokens: the new token ids up to and including the first EOS (what generate() returns for the request's
-    row before it pads); with num_return_sequences = n > 1, a list of n such lists, sample 0 first."""
+    row before it pads); with num_return_sequences = n > 1, a list of n such lists, sample 0 first.
+    logprobs: with generate_batch(return_logprobs=True), one float per generated token (one list per sample when n > 1):
+    log_softmax of the scores the token was picked from, at the token; empty otherwise."""
     request_id: str
     prompt_ids: List[int]
     generated_tokens: list
+    logprobs: list = field(default_factory=list)
 
 
 _BATCH_REQUEST_KEYS = ("images", "input_ids", "question_ids", "max_new_tokens", "seed", "request_id")
@@ -549,14 +553,45 @@ class U2MetaForCausalLM(ABC):
         if num_beams != 1:
             beam = self._generate_beam_search(kwargs, gc, num_beams, bool(do_sample), n_ret, pad)
         procs = self._generate_logits_processors(kwargs, gc, L, eos, eng.g.vocab_size)
+        return_dict, want_scores, want_logits = self._generate_output_flags(kwargs, gc)
         self._check_remaining_generate_kwargs(kwargs)
         if n_ret > 1 and not do_sample and beam is None:
             raise ValueError("num_return_sequences > 1 needs do_sample=True (greedy decoding is deterministic; HF raises too)")
         ids = eng.generate(inputs_embeds.to(torch.bfloat16), max_new_tokens=max_new, eos_token_id=eos,
                            do_sample=bool(do_sample), temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
-                           num_return_sequences=n_ret, lengths=lengths, processors=procs, beam=beam)
-        if beam is not None:
-            return ids  # HF's beam output: best hypotheses first, each filled after its end with pad or eos[0]
+                           num_return_sequences=n_ret, lengths=lengths, processors=procs, beam=beam,
+                           output_scores=want_scores, output_logits=want_logits)
+        scores = logits = None
+        if want_scores or want_logits:
+            ids, scores, logits = ids
+        if beam is None:
+            ids = self._generate_mask_after_eos(ids, eos, pad)
+        if not return_dict:
+            return ids
+        steps = lambda buf: None if buf is None else tuple(buf[t] for t in range(ids.shape[1]))
+        if beam is None:
+            return GenerateDecoderOnlyOutput(sequences=ids, scores=steps(scores), logits=steps(logits))
+        return GenerateBeamDecoderOnlyOutput(
+            sequences=ids, sequences_scores=eng.last_beam_scores.to(ids.device) if want_scores else None,
+            scores=steps(scores), logits=steps(logits), beam_indices=eng.last_beam_indices)
+
+    @staticmethod
+    def _generate_output_flags(kwargs: dict, generation_config) -> Tuple[bool, bool, bool]:
+        """return_dict_in_generate, output_scores and output_logits, popped from `kwargs`, else read from
+        `generation_config`. HF keeps scores and logits only in a returned dict, so without it both are False."""
+        def flag(name):
+            v = kwargs.pop(name, None)
+            if v is None and generation_config is not None:
+                v = getattr(generation_config, name, None)
+            return bool(v)
+        return_dict = flag("return_dict_in_generate")
+        scores, logits = flag("output_scores"), flag("output_logits")
+        return return_dict, scores and return_dict, logits and return_dict
+
+    @staticmethod
+    def _generate_mask_after_eos(ids: torch.Tensor, eos, pad) -> torch.Tensor:
+        """generate()'s greedy / sampled ids: every position after a row's first EOS becomes pad (eos[0] when pad is
+        None), and the columns after the last row's first EOS are dropped, as HF's stopping criteria end the loop."""
         if eos:
             hit = torch.isin(ids, torch.as_tensor(eos, device=ids.device))
             after = (hit.cumsum(dim=1) - hit.long()) > 0  # strictly after the first EOS
@@ -575,8 +610,10 @@ class U2MetaForCausalLM(ABC):
         or [1, L], unpadded) and optionally `question_ids`, `max_new_tokens`, `seed` and `request_id` (default: the
         request's index as a string); it is read lazily, so only the requests in the decode rows are held.
         num_slots: decode rows in flight (default and maximum: the rows one decode step carries, 16 on the wgmma path).
-        kwargs: generate()'s greedy / sampling / num_return_sequences / logits-processor / eos / pad options. Request i
-        without a seed samples with seed + i. Returns {request_id: GenerationOutput}."""
+        kwargs: generate()'s greedy / sampling / num_return_sequences / logits-processor / eos / pad options, and
+        return_logprobs (HF's ContinuousBatchingConfig name): each output's `logprobs` then holds the log-prob of every
+        generated token, recorded inside the decode step. Request i without a seed samples with seed + i. Returns
+        {request_id: GenerationOutput}."""
         eng = self.engine()
         gc = getattr(self, "generation_config", None)
         head = self._generate_batch_head(kwargs, gc, num_slots, eng._decode_rows(), eng.g.vocab_size)
@@ -606,9 +643,13 @@ class U2MetaForCausalLM(ABC):
         out = eng.generate_continuous(engine_requests(), head["num_slots"], eos_token_id=head["eos"],
                                       pad_token_id=head["pad"], do_sample=head["do_sample"],
                                       temperature=head["temperature"], top_k=head["top_k"], top_p=head["top_p"],
-                                      num_return_sequences=head["n"], processors=head["processors"])
-        return {rid: GenerationOutput(rid, prompts[rid], seqs[0] if head["n"] == 1 else seqs)
-                for rid, seqs in out.items()}
+                                      num_return_sequences=head["n"], processors=head["processors"],
+                                      return_logprobs=head["return_logprobs"])
+        one = (lambda x: x[0]) if head["n"] == 1 else (lambda x: x)
+        if not head["return_logprobs"]:
+            return {rid: GenerationOutput(rid, prompts[rid], one(seqs)) for rid, seqs in out.items()}
+        return {rid: GenerationOutput(rid, prompts[rid], one([t for t, _ in res]), one([lp for _, lp in res]))
+                for rid, res in out.items()}
 
     def _generate_batch_head(self, kwargs: dict, gc, num_slots, rows: int, vocab_size: int) -> dict:
         """generate_batch()'s options, read and validated by generate()'s helpers and generation_config fallbacks."""
@@ -646,6 +687,7 @@ class U2MetaForCausalLM(ABC):
         if not min_new_set and (kwargs.get("min_length") or getattr(gc, "min_length", None) or 0) > 0:
             raise NotImplementedError("generate_batch(): min_length counts each prompt's width; pass min_new_tokens")
         procs = self._generate_logits_processors(kwargs, gc, 0, eos, vocab_size)
+        return_logprobs = bool(opt("return_logprobs", False))
         self._check_remaining_generate_kwargs(kwargs)
         if n_ret > 1 and not do_sample:
             raise ValueError("num_return_sequences > 1 needs do_sample=True (greedy decoding is deterministic; HF raises too)")
@@ -658,7 +700,8 @@ class U2MetaForCausalLM(ABC):
             raise ValueError(f"generate_batch() supports at most {_lib.LP_MAX_EOS} EOS ids, got {len(eos)}")
         return dict(num_slots=int(S), n=n_ret, do_sample=bool(do_sample), temperature=temperature, top_k=top_k,
                     top_p=top_p, seed=int(seed), max_new_tokens=max_new, max_length=int(max_length), eos=eos,
-                    pad=int(pad) if pad is not None else (eos[0] if eos else 0), processors=procs)
+                    pad=int(pad) if pad is not None else (eos[0] if eos else 0), processors=procs,
+                    return_logprobs=return_logprobs)
 
     @staticmethod
     def _generate_batch_request(i: int, r, seed: int) -> dict:

@@ -786,10 +786,13 @@ def logits_process_slots(logits: torch.Tensor, params: torch.Tensor, ids: torch.
 
 
 def slot_update(ids: torch.Tensor, slots: torch.Tensor, out: torch.Tensor, params: torch.Tensor,
-                length: Optional[torch.Tensor] = None, length_plus1: Optional[torch.Tensor] = None) -> None:
+                length: Optional[torch.Tensor] = None, length_plus1: Optional[torch.Tensor] = None,
+                lp: Optional[tuple] = None) -> None:
     """Slot bookkeeping after a pick (u2_slot_update): every decoding slot appends ids[b] to out[b] at its count,
     counts it, finishes on an EOS id or max_new_tokens and, when the cache lengths are given, advances them; every
-    finished slot gets ids[b] = pad. ids int64 [B] (contiguous), out int64 [B, width], params: slot_params()."""
+    finished slot gets ids[b] = pad. ids int64 [B] (contiguous), out int64 [B, width], params: slot_params().
+    lp (optional): (the step's log-probs fp32 [B], fp32 [B, width] like out): each live slot also appends its
+    log-prob (u2_slot_update_lp)."""
     _need_cuda(ids, slots, out, params, length, length_plus1)
     B = ids.numel()
     if ids.dtype != torch.int64 or not ids.is_contiguous():
@@ -802,9 +805,95 @@ def slot_update(ids: torch.Tensor, slots: torch.Tensor, out: torch.Tensor, param
     for t in (length, length_plus1):
         if t is not None and (t.dtype != torch.int32 or t.numel() != B or not t.is_contiguous()):
             raise ValueError("slot_update: length / length_plus1 must be contiguous int32 [B]")
-    _lib.check(_lib.load().u2_slot_update(ids.data_ptr(), B, slots.data_ptr(), out.data_ptr(), out.stride(0),
-                                          params.data_ptr(), _ptr(length), _ptr(length_plus1), _stream()),
-               "u2_slot_update")
+    if lp is None:
+        _lib.check(_lib.load().u2_slot_update(ids.data_ptr(), B, slots.data_ptr(), out.data_ptr(), out.stride(0),
+                                              params.data_ptr(), _ptr(length), _ptr(length_plus1), _stream()),
+                   "u2_slot_update")
+        return
+    lp_in, lp_out = lp
+    _need_cuda(lp_in, lp_out)
+    if lp_in.dtype != F32 or lp_in.numel() != B or not lp_in.is_contiguous():
+        raise ValueError("slot_update: the step's log-probs must be contiguous fp32 [B]")
+    if lp_out.dtype != F32 or lp_out.shape != out.shape or lp_out.stride() != out.stride():
+        raise ValueError("slot_update: the log-prob rows must be fp32 shaped and strided like out")
+    _lib.check(_lib.load().u2_slot_update_lp(ids.data_ptr(), B, slots.data_ptr(), out.data_ptr(), out.stride(0),
+                                             lp_in.data_ptr(), lp_out.data_ptr(), params.data_ptr(), _ptr(length),
+                                             _ptr(length_plus1), _stream()), "u2_slot_update_lp")
+
+
+def row_store_params(device, dst_ptr: int, ld_step: int, ld_row: int, steps: int,
+                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The u2_row_store_params block (include/u2b200.h) in device memory, as uint8: row r of step t goes to the fp32
+    element dst_ptr + t * ld_step + r * ld_row (in elements), for 0 <= t < steps. `out` (a block made earlier) is
+    overwritten in place, so a captured decode step stores into a new call's buffer without a new capture."""
+    blk = _lib.RowStoreParams()
+    blk.dst, blk.ld_step, blk.ld_row, blk.steps = int(dst_ptr), int(ld_step), int(ld_row), int(steps)
+    host = torch.frombuffer(bytearray(bytes(blk)), dtype=torch.uint8)
+    if out is None:
+        return host.to(device)
+    out.copy_(host)
+    return out
+
+
+def row_store_dst(buf: torch.Tensor) -> dict:
+    """row_store_params() arguments that store step t's rows into buf[t] of an fp32 [steps, rows, V] view (unit column
+    stride)."""
+    if buf.dtype != F32 or buf.dim() != 3 or buf.stride(2) != 1 or not buf.is_cuda:
+        raise ValueError("row store: the destination must be a CUDA fp32 [steps, rows, V] view with unit column stride")
+    return dict(dst_ptr=buf.data_ptr(), ld_step=buf.stride(0), ld_row=buf.stride(1), steps=buf.shape[0])
+
+
+def _check_row_store(params: Optional[torch.Tensor]):
+    if params is not None and (params.dtype != torch.uint8 or params.numel() != C.sizeof(_lib.RowStoreParams)):
+        raise ValueError("params must be the block of row_store_params()")
+
+
+def store_rows(src: torch.Tensor, params: torch.Tensor, *, step: int = 0, step_dev=None) -> None:
+    """Copies fp32 src [rows, V] to the rows of step t = *step_dev (or step) of the row_store_params() destination."""
+    _need_cuda(src, params, step_dev)
+    if src.dtype != F32 or src.dim() != 2 or src.stride(1) != 1:
+        raise TypeError("store_rows: src must be fp32 [rows, V] with unit column stride")
+    _check_row_store(params)
+    _lib.check(_lib.load().u2_store_rows_f32(src.data_ptr(), src.shape[0], src.shape[1], src.stride(0),
+                                             params.data_ptr(), _ptr(step_dev), int(step), _stream()),
+               "u2_store_rows_f32")
+
+
+def sample_out(logits: torch.Tensor, params: torch.Tensor, out: torch.Tensor, *, scores: Optional[torch.Tensor] = None,
+               logprob: Optional[torch.Tensor] = None, step: int = 0, step_dev=None,
+               slots: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """sample_dev() (or sample_slots() when `slots` is given) with the same draw, that also writes the warped scores row
+    into the row_store_params() destination `scores` and the pick's log-prob into logprob fp32 [B], each when given."""
+    _need_cuda(logits, params, out, scores, logprob, step_dev, slots)
+    B, V = logits.shape
+    if params.dtype != torch.uint8 or params.numel() != 24:
+        raise ValueError("sample_out: params must be the 24-byte block of sample_params()")
+    _check_row_store(scores)
+    if slots is not None:
+        _check_slots(slots, B)
+    if logprob is not None and (logprob.dtype != F32 or logprob.numel() != B or not logprob.is_contiguous()):
+        raise ValueError("sample_out: logprob must be contiguous fp32 [B]")
+    _lib.check(_lib.load().u2_sample_out_f32(logits.data_ptr(), out.data_ptr(), B, V, logits.stride(0),
+                                             params.data_ptr(), _ptr(step_dev), int(step), _ptr(slots), _ptr(scores),
+                                             _ptr(logprob), _stream()), "u2_sample_out_f32")
+    return out
+
+
+def pick_logprob(logits: torch.Tensor, ids: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[b] = log_softmax(logits[b])[ids[b]], fp32 [B]."""
+    _need_cuda(logits, ids, out)
+    B, V = logits.shape
+    if logits.dtype != F32 or logits.stride(1) != 1:
+        raise TypeError("pick_logprob: logits must be fp32 with unit column stride")
+    if ids.dtype != torch.int64 or ids.numel() != B or not ids.is_contiguous():
+        raise ValueError("pick_logprob: ids must be contiguous int64 [B]")
+    if out is None:
+        out = torch.empty(B, device=logits.device, dtype=F32)
+    if out.dtype != F32 or out.numel() != B or not out.is_contiguous():
+        raise ValueError("pick_logprob: out must be contiguous fp32 [B]")
+    _lib.check(_lib.load().u2_pick_logprob_f32(logits.data_ptr(), B, V, logits.stride(0), ids.data_ptr(),
+                                               out.data_ptr(), _stream()), "u2_pick_logprob_f32")
+    return out
 
 
 def log_softmax(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
